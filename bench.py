@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""bench.py -- decoder tokens/sec of the nats hot path (BASELINE.json metric) on N B200s of one node.
+"""bench.py -- decoder tokens/sec of the nats hot path (BASELINE.json metric) on N H100s of one node.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload c3|c2|c5] [--ragged]
+                    [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 Workloads (BASELINE.json configs):
@@ -53,7 +54,25 @@ WORKLOADS = {
     'c5': dict(Tx=801, Ty=100, dim=1000, dim_word=100, dim_att=100, n_words=30000, B=10,
                name='gen_sample beam search: beam=10, src_len=800, dim=1000, |V|=30000, kl=ctx=state factor 1.0'),
 }
-METRIC = 'decoder tokens/sec (dim=1000, src=400, |V|=30k) @1/2/4/8 B200 vs Theano CPU'
+METRIC = 'decoder tokens/sec (dim=1000, src=400, |V|=30k) @1/2/4/8 H100 vs Theano CPU'
+
+
+DUMP_SAMPLE = 1 << 20          # elements kept of an output larger than this (fixed seeded positions)
+
+
+def dump_outputs(d, arrays):
+    """Write what the timed path returned in its last step as DIR/<name>.npy (float32, or float64 for tokens and scores).
+    Outputs above DUMP_SAMPLE elements are sampled at positions drawn from a fixed seed (also written, as <name>_index),
+    so two builds can be compared output for output; the whole dump stays far below 64 MB."""
+    os.makedirs(d, exist_ok=True)
+    for name, a in arrays.items():
+        a = np.asarray(a)
+        a = a.astype('float64') if a.dtype.kind in 'iuf' and a.dtype.itemsize == 8 else a.astype('float32')
+        if a.size > DUMP_SAMPLE:
+            idx = np.sort(np.random.RandomState(0).choice(a.size, DUMP_SAMPLE, replace=False))
+            np.save(os.path.join(d, name + '_index.npy'), idx.astype('float64'))
+            a = a.reshape(-1)[idx]
+        np.save(os.path.join(d, name + '.npy'), a)
 
 
 def make_batches(w, n, seed, B=None, ragged=False):
@@ -85,11 +104,11 @@ def load_peaks():
         with open(p) as f:
             d = json.load(f)
         return d.get('hbm_gbs', 6650.0), d.get('bf16_tflops_sustained', 1400.0), 'measured (MEASURED_PEAKS.json)'
-    return 6650.0, 1400.0, 'fallback (B200_PROFILING.md)'
+    return 3350.0, 495.0, 'NVIDIA H100 SXM data sheet (HBM3 3.35 TB/s, dense TF32 495 TFLOP/s), not measured'
 
 
 class ClockSampler(object):
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region."""
     Q = ('clocks.sm,clocks.max.sm,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,'
          'clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap')
 
@@ -136,7 +155,7 @@ _BLAS_CHOICE = {}
 
 
 def best_blas_threads(w=None):
-    """OpenBLAS with every host thread (128 on the B200 boxes) is pathologically slow on the skinny products of the
+    """OpenBLAS with every host thread is pathologically slow on the skinny products of the
     recurrence; pick the thread count that is fastest on a SHORT real piece of the workload (a forward + backward pass of
     the restatement at the workload's dim / |V| / batch with src_len 40, tgt_len 6) so that the CPU baseline is a fair one."""
     try:
@@ -402,7 +421,7 @@ def beam_run(nats, tparams, opts, w, steps, warm=True, kernels=False):
         torch.cuda.synchronize()
         t_init = time.time() - t1
         t0 = time.time()
-        nats.gen_sample(tparams, f_init, f_next, x, opts, None, 10, steps, False, False, True, 1.0, 1.0, 1.0)
+        result = nats.gen_sample(tparams, f_init, f_next, x, opts, None, 10, steps, False, False, True, 1.0, 1.0, 1.0)
         torch.cuda.synchronize()
         dt = time.time() - t0
     finally:
@@ -411,6 +430,11 @@ def beam_run(nats, tparams, opts, w, steps, warm=True, kernels=False):
     out = {'ms_per_step': (dt - t_init) / steps * 1e3, 'f_init_ms': t_init * 1e3, 'steps': steps, 'sentence_ms': dt * 1e3,
            'hyp_tokens_per_s': live / max(dt - t_init, 1e-9),
            'how': 'gen_sample wall clock (host bookkeeping included) minus one f_init; beam 10, src_len %d, kl=ctx=state=1' % (w['Tx'] - 1)}
+    samples, scores = result[0], result[1]
+    toks = np.full((len(samples), max([len(s) for s in samples] + [1])), -1.0)
+    for i, s in enumerate(samples):
+        toks[i, :len(s)] = s
+    outputs = {'beam_tokens': toks, 'beam_scores': np.asarray(scores, 'float64')}
     if kernels:
         # the same sentence under the CUPTI activity trace: launches and exclusive device time per kernel
         tparams['ff_logit_b'].set_value(bmod)
@@ -426,7 +450,7 @@ def beam_run(nats, tparams, opts, w, steps, warm=True, kernels=False):
                           'gpu_busy_us_per_step_incl_f_init': busy / steps,
                           'top': [{'kernel': k_.replace('(anonymous namespace)::', '').replace('nats::', '').replace('void ', '').split('(')[0][:60],
                                    'excl_us': round(v[0], 1), 'launches': v[2]} for k_, v in top]}
-    return out
+    return out, outputs
 
 
 def gen_throughput(nats, tparams, opts, w, n_sent=32, steps=25):
@@ -476,7 +500,10 @@ def main():
     ap.add_argument('--no-cpu-baseline', action='store_true')
     ap.add_argument('--no-regions', action='store_true', help='skip the R1 (decoder forward) / R3 (beam step) measurements')
     ap.add_argument('--no-kernels', action='store_true', help='skip the CUPTI per-kernel table')
+    ap.add_argument('--dump-outputs', metavar='DIR', help='write the outputs of the last timed step to DIR/<name>.npy')
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error('--steps must be >= 1')
     w = WORKLOADS[args.workload]
     rank = int(os.environ.get('RANK', '0'))
     world = int(os.environ.get('WORLD_SIZE', '1'))
@@ -489,7 +516,7 @@ def main():
                         'train step: f_grad_shared + f_update (nats.py:1400-1411)',
               'global_batch': w['B'] * max(world, 1), 'src_len': w['Tx'] - (1 if beam else 0), 'tgt_len': w['Ty'],
               'parallelism': 'dp%d' % max(world, 1),
-              'l2_policy': 'per-step working set (saved activations + weights, > 2 GB) exceeds the 126 MB L2'}
+              'l2_policy': 'per-step working set (saved activations + weights, > 2 GB) exceeds the 50 MB L2'}
     if not beam:
         config.update({'optimizer': 'adadelta', 'clip_c': 100.0})
 
@@ -536,11 +563,13 @@ def main():
     if beam:
         if rank != 0:
             return 0
-        K = max(args.steps, 4)
+        K = args.steps
         clk = ClockSampler(local)
         t0 = time.time()
-        r = beam_run(nats, tparams, opts, w, K, kernels=not args.no_kernels)
-        full = beam_run(nats, tparams, opts, w, 100, warm=False)
+        r, outputs = beam_run(nats, tparams, opts, w, K, kernels=not args.no_kernels)
+        if args.dump_outputs:
+            dump_outputs(args.dump_outputs, outputs)
+        full = beam_run(nats, tparams, opts, w, 100, warm=False)[0]
         clocks = clk.stop(t0, time.time())
         Tx5, k5 = w['Tx'], 10
         d2h_sentence = 2 * k5 * K * Tx5 * 4 + 2 * k5 * K * 4 + 3 * k5 * 4 + 32     # attention histories (live + retired), tokens, scores, counters
@@ -647,6 +676,10 @@ def main():
         ev1.record()
         barrier()
         dev_ms = max_over_ranks(ev0.elapsed_time(ev1))
+    if args.dump_outputs and rank == 0:
+        # the last timed step's results: per-sentence costs, the flat gradient and the parameters after the update
+        dump_outputs(args.dump_outputs, {'cost': plan.cost.cpu().numpy(), 'grads': graph.grads[:tparams.total].cpu().numpy(),
+                                         'params': tparams.flat.cpu().numpy()})
     t_wall1 = time.time()
     clocks = clk.stop(t_wall0, t_wall1) if clk is not None else None
 
@@ -689,7 +722,7 @@ def main():
     r3 = None
     if world == 1 and args.workload == 'c3' and not args.no_regions:
         try:
-            r3 = beam_run(nats, tparams, opts, WORKLOADS['c5'], 20)
+            r3 = beam_run(nats, tparams, opts, WORKLOADS['c5'], 20)[0]
             r3['gen_stream'] = gen_throughput(nats, tparams, opts, WORKLOADS['c5'])      # sentences/s of the gen driver's loop
         except Exception as e:
             r3 = {'error': repr(e)}
@@ -743,21 +776,14 @@ def roofline_of(cls, w, step_ms):
     us = k['us_per_launch']
     base = {'kernel': name, 'share_of_step': k['ms_per_step'] / step_ms, 'us_per_launch': us, 'peak_source': src,
             'duration_source': 'CUPTI activity trace of the replayed graph step'}
-    traffic = None                                            # dram bytes per launch from the committed ncu --set full capture
-    try:
-        with open(os.path.join(os.path.dirname(os.path.abspath(__file__)), 'profiles', 'ncu_traffic.json')) as f:
-            t = json.load(f).get(name)
-        if t and (t.get('Tx'), t.get('B'), t.get('dim')) == (w['Tx'], w['B'], w['dim']):
-            traffic = t['dram_bytes_per_launch']
-    except (OSError, ValueError, KeyError):
-        pass
+    traffic = None
     if name.startswith('enc_tc'):
         flops = 2.0 * 2 * (Tx - 1) * B * D * 3 * D            # both directions, fp32-equivalent (each is 3 tf32 products)
         ach = flops / (us * 1e-6) / 1e12
         base.update({'bound': 'tensor', 'achieved': ach, 'peak': tf, 'unit': 'TFLOP/s', 'frac': ach / tf,
                      'algo_flops_per_launch': flops, 'traffic': traffic,
                      'limiter': 'inter-SM dependency latency: 2 L2 exchange hops per recurrent step (K partials, then h_t / dG_t); '
-                                'the tensor pipe itself is busy ~1/3 of the step (84 tcgen05 MMAs of 3xTF32 per CTA and step)',
+                                'the tensor pipe itself is busy a fraction of the step (3xTF32 wgmma per k-step, 189 x 32 x 256 per CTA and step)',
                      'us_per_recurrent_step': us / Tx})
         return base
     if name.startswith('tc_gemm'):
@@ -765,7 +791,7 @@ def roofline_of(cls, w, step_ms):
         ach = gf / k['ms_per_step'] if gf else None          # GFLOP / ms = TFLOP/s
         base.update({'bound': 'tensor', 'achieved': ach, 'peak': tf, 'unit': 'TFLOP/s', 'frac': ach / tf if ach else None, 'traffic': None,
                      'algo_gflop_per_step': gf,
-                     'note': 'fp32-equivalent flops: every product is 3 tf32 tcgen05 MMAs (3xTF32), so the tensor pipe executes 3x this'})
+                     'note': 'fp32-equivalent flops: every product is 3 tf32 wgmma MMAs (3xTF32), so the tensor pipe executes 3x this'})
         return base
     C = 2 * D
     bytes_per_launch = {'att_context': 4.0 * (Tx * B * C + 3 * B * C + 3 * B * Tx), 'att_bwd_dalpha': 4.0 * (Tx * B * C + 2 * B * C + B * Tx)}.get(name)

@@ -1,5 +1,5 @@
 /*
- * nats_b200.h -- C ABI of libnats_b200.so: the B200 (sm_100a) implementation of the hot path of
+ * nats_b200.h -- C ABI of libnats_b200.so: the H100 (sm_90a) implementation of the hot path of
  * lukecq1231/nats (scripts/nats.py).
  *
  * The reference has no FFI layer: its operator boundary is the set of compiled `theano.function`
@@ -254,8 +254,9 @@ int nats_beam_step(nats_ctx_t* ctx, void* stream, const nats_dims_t* dims, const
 
 /* ---------------------------------------------------------------- diagnostics ------------------- */
 /* The library's internal GEMM engine, exposed for the parity tests: C = op(A).op(B) (+bias) (+C), row-major,
- * path 0 = exact-fp32 FFMA kernels, path 1 = tcgen05 3xTF32 kernel with software loaders, path 2 = tcgen05 3xTF32
- * kernel fed by TMA (needs 16-byte aligned operands, leading dimensions multiple of 4).  splitk > 1 writes splitk slabs
+ * path 0 = exact-fp32 FFMA kernels, path 1 = wgmma 3xTF32 kernel with software loaders, path 2 = wgmma 3xTF32 kernel
+ * fed by TMA (needs 16-byte aligned operands, leading dimensions multiple of 4), path 3 = the TMA-fed kernel with the
+ * 128-row operand split in registers (its default for skinny products).  splitk > 1 writes splitk slabs
  * of M*ldc floats to C (the consumer kernels sum them); batch > 1 uses the given strides. */
 int nats_debug_gemm(nats_ctx_t* ctx, void* stream, int path, int transA, int transB, int M, int N, int K,
                     const float* A, int lda, const float* B, int ldb, float* C, int ldc, const float* bias,

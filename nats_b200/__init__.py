@@ -1,4 +1,4 @@
-"""nats_b200 -- B200-native (sm_100a) implementation of the hot path of lukecq1231/nats.
+"""nats_b200 -- H100-native (sm_90a) implementation of the hot path of lukecq1231/nats.
 
     from nats_b200 import nats          # the reference-compatible module (scripts/nats.py surface)
 

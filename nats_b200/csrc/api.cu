@@ -82,8 +82,8 @@ int nats_ctx_create(int device, nats_ctx_t** out) {
     NATS_CUDA_OK(cudaSetDevice(device));
     cudaDeviceProp prop;
     NATS_CUDA_OK(cudaGetDeviceProperties(&prop, device));
-    if (prop.major < 10) {
-        set_error("libnats_b200 is built for sm_100a only; device %d is sm_%d%d", device, prop.major, prop.minor);
+    if (prop.major != 9 || prop.minor != 0) {
+        set_error("libnats_b200 is built for sm_90a only; device %d is sm_%d%d", device, prop.major, prop.minor);
         return 3;
     }
     nats_ctx* c = new nats_ctx;
@@ -100,9 +100,7 @@ int nats_ctx_create(int device, nats_ctx_t** out) {
     enc_tc_enable(getenv("NATS_ENC_TC") ? atoi(getenv("NATS_ENC_TC")) : 1);      // 0: per-step encoder path, 2 / 3: forward / backward only
     attention_set_cc_keep(getenv("NATS_CC_KEEP") ? atoi(getenv("NATS_CC_KEEP")) : 0);
     tma_gemm_set_ts(getenv("NATS_TS") ? atoi(getenv("NATS_TS")) : 1);
-    if (getenv("NATS_GEMM_DBG")) tma_gemm_debug_mode(atoi(getenv("NATS_GEMM_DBG")));
     if (getenv("NATS_TRACE_GATES")) gates_trace(atoi(getenv("NATS_TRACE_GATES")));
-    if (getenv("NATS_TRACE")) { tma_gemm_trace(atoi(getenv("NATS_TRACE"))); }
     pdl_set(getenv("NATS_PDL") ? atoi(getenv("NATS_PDL")) : 1);
     gemm_set_tensor_cores(getenv("NATS_TC") ? atoi(getenv("NATS_TC")) : 2);
     if (r != 0) { cudaFree(c->dev_scratch); delete c; return r; }
@@ -190,7 +188,7 @@ int nats_debug_gemm(nats_ctx_t* ctx, void* stream, int path, int transA, int tra
     if (splitk > 1) gemm_set_split(p, splitk, (long long)M * ldc);
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     if (path == 1) return tc_gemm_launch(st, &p, 1, transA != 0, transB != 0);
-    if (path == 2 || path == 3) {        // 3 = TMA-fed with the 128-row operand in tensor memory (skinny shapes)
+    if (path == 2 || path == 3) {        // 3 = TMA-fed with the 128-row operand through registers (skinny shapes)
         NATS_REQUIRE(tma_gemm_eligible(&p, 1), "operands not TMA-compatible (alignment)");
         const int keep_ts = tma_gemm_get_ts();
         tma_gemm_set_ts(path == 3 ? 1 : 0);

@@ -1,9 +1,9 @@
-"""Build libnats_b200.so in-tree with nvcc for sm_100a (cross-compiles without a GPU).
+"""Build libnats_b200.so in-tree with nvcc for sm_90a (cross-compiles without a GPU).
 
     python nats_b200/csrc/build.py [--force]
 
-Every translation unit is compiled with `-gencode arch=compute_100a,code=sm_100a -lineinfo`; objects go to
-nats_b200/csrc/build/, the shared library to nats_b200/libnats_b200.so (git-ignored, shipped to the GPU box).
+Every translation unit is compiled with `-gencode arch=compute_90a,code=sm_90a -lineinfo`; objects go to
+nats_b200/csrc/build/, the shared library to nats_b200/libnats_b200.so (both git-ignored build products).
 """
 import hashlib
 import os
@@ -21,7 +21,7 @@ SOURCES = ['gemm.cu', 'tc_gemm.cu', 'tma_gemm.cu', 'enc_tc.cu', 'ops_elem.cu', '
 HEADERS = ['common.cuh', 'prof.cuh', 'tc_common.cuh', 'gemm.cuh', 'gates.cuh', 'ops.cuh', 'workspace.cuh', 'model.cuh',
            os.path.join(ROOT, 'include', 'nats_b200.h')]
 NVCC = os.environ.get('NVCC', '/usr/local/cuda/bin/nvcc')
-FLAGS = os.environ.get('NATS_NVCC_EXTRA', '').split() + ['-gencode', 'arch=compute_100a,code=sm_100a', '-O3', '-lineinfo', '-std=c++17',
+FLAGS = os.environ.get('NATS_NVCC_EXTRA', '').split() + ['-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-lineinfo', '-std=c++17',
          '-Xcompiler', '-fPIC', '-Xcompiler', '-fvisibility=hidden']
 
 
@@ -51,7 +51,7 @@ def build(force=False, verbose=True):
 
     with ThreadPoolExecutor(max_workers=min(8, len(SOURCES))) as ex:
         objs = list(ex.map(cc, SOURCES))
-    cmd = [NVCC, '-shared', '-o', OUT] + objs + ['-gencode', 'arch=compute_100a,code=sm_100a', '-lcudart']
+    cmd = [NVCC, '-shared', '-o', OUT] + objs + ['-gencode', 'arch=compute_90a,code=sm_90a', '-lcudart']
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError('link failed:\n%s\n%s' % (r.stdout, r.stderr))

@@ -1,4 +1,4 @@
-// common.cuh -- shared helpers for libnats_b200 (sm_100a).  Not part of the C ABI.
+// common.cuh -- shared helpers for libnats_b200 (sm_90a).  Not part of the C ABI.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

@@ -1,29 +1,27 @@
 // enc_tc.cu -- the bidirectional GRU encoder recurrence (nats.py:336-372, both directions) and its reverse mode as ONE
-// persistent, WEIGHT-STATIONARY tcgen05 kernel per pass.
+// persistent, WEIGHT-STATIONARY tensor-core kernel per pass.
 //
-// Why.  A recurrent step is  h[n,D] x [U|Ux][D,3D]  with n = 32: launched per step it cost 11.7 us forward / 16 us
-// backward (split-K product kernel + gate kernel, two kernel boundaries, 24 MB of weights re-streamed from L2 per step)
-// and the 2 x 400 dependent steps were 67 % of the training step.  Here the weights never move after the prologue:
-//   * one CTA per SM, 72 CTAs per direction (144 of the 148 SMs at D = 1000).  The swapped product (rows = weight
-//     columns, N = batch) is cut into tiles of <= 128 rows x Kc <= 352 deep:
-//       forward : 24 row tiles (the r|u|c gate columns of 42 hidden units each) x 3 K chunks of D;
-//       backward:  8 row tiles (125 hidden units of d h_{t-1})                  x 9 K chunks of 3D.
-//   * each CTA keeps its tile of [U|Ux] (forward) / [U|Ux]^T (backward) as RAW fp32 in shared memory in the canonical
-//     K-major SWIZZLE_128B UMMA layout (176 KB) -- the tensor core truncates fp32 words to tf32, so the raw tile IS the
-//     "hi" operand -- and the residual  lo = x - trunc_tf32(x)  of the same tile in TENSOR MEMORY (352 of the 512
-//     columns).  3xTF32 per k-step of 8:   acc[hi.hi | hi.lo] += A_raw(smem) x [B_raw | B_lo]  (one N-stacked MMA),
-//     acc[lo.hi] += A_lo(tmem) x B_raw.   84 MMAs per step and CTA, no per-step split pass, no weight traffic at all.
+// Why.  A recurrent step is  h[n,D] x [U|Ux][D,3D]  with n = 32: launched per step it costs a split-K product kernel + a
+// gate kernel, two kernel boundaries and 24 MB of weights re-streamed from L2 per step, and the 2 x 400 dependent steps
+// dominate the training step.  Here the weights never move after the prologue:
+//   * one CTA per SM, at most 66 CTAs per direction on the 132 SMs of an H100.  The swapped product (rows = weight columns,
+//     N = batch) is cut into row tiles of <= 192 rows (three warpgroups of 64) x Kc deep; at D = 1000:
+//       forward : 16 row tiles (the r|u|c gate columns of 63 hidden units each) x 4 K chunks of D;
+//       backward:  8 row tiles (125 hidden units of d h_{t-1})                  x 8 K chunks of 3D.
+//   * each CTA keeps its tile of [U|Ux] (forward) / [U|Ux]^T (backward) as RAW fp32 in shared memory in the K-major
+//     SWIZZLE_128B layout of the wgmma descriptors (<= 192 KB).  The tensor core reads the upper 19 bits of an fp32 word,
+//     so the raw tile IS the "hi" operand; its residual  lo = x - trunc_tf32(x)  is formed in registers from the same
+//     shared-memory words right before each k-step and fed as the register A operand.  3xTF32 per k-step of 8:
+//       acc_hh += A_raw(smem) x B_raw,   acc_x += A_raw(smem) x B_lo  +  A_lo(registers) x B_raw.
 //   * per step the only moving operand is B = h_{t-1} (forward; raw = the context row itself) / dG_{t+1} (backward; raw =
-//     the saved gate-derivative row itself), plus its residual in a 2-deep side buffer written by the producers: TMA
-//     boxes of 32 k x n rows into a 6-stage ring, gated by ONE monotonic counter per direction in L2 (red.release /
+//     the saved gate-derivative row itself), plus its residual in a 2-deep side buffer written by the gate warps: TMA
+//     boxes of 32 k x n rows into a ring of stages, gated by ONE monotonic counter per row tile in L2 (red.release /
 //     ld.acquire).
 //   * the K partials of a row tile are exchanged through L2 (fixed summation order: deterministic): every CTA writes
 //     its partial slab, bumps the tile's counter, waits for its S-1 peers and finishes the gate arithmetic (forward:
 //     nats.py:336-356; backward: its reverse) for ITS share of the tile's units in registers; it stores h_t straight
 //     into the concatenated context [Tx,n,2D] (nats.py:713 needs no copy) / dG_t into the saved arrays the weight-gradient
-//     products read, publishes the residuals, bumps the direction counter, and only then writes what nobody waits for.
-//     (Clusters + distributed shared memory would save ~0.4 us per step, but only 45 clusters of 3 are co-resident on a
-//     B200 with this footprint -- 48 are needed -- so the exchange goes through L2.)
+//     products read, publishes the residuals, bumps the counter, and only then writes what nobody waits for.
 // Every spin is bounded (a stuck CTA traps after ~1 s instead of hanging the GPU).  The grid must be co-resident: the
 // host checks the occupancy before choosing this path.
 #include <cuda.h>
@@ -37,15 +35,17 @@ namespace {
 
 using namespace tc;
 
-#ifndef ENC_TC_DBG
-#define ENC_TC_DBG 0        // timing experiments of tools/micro/enc_tc_test.cu (WRONG results): 1 = weight tile not advanced, 2 = no shared-memory-A MMAs, 3 = no tensor-memory-A MMAs
-#endif
-constexpr int kGateWarp0 = 7;           // warps 0-3: TMEM lane quadrants -> K-partial words; 4: flag poll + TMA producer;
-constexpr int kGateThreads = 256;       // 5 / 6: MMA issuers (A from shared / A from tensor memory); 7-14: gates
+constexpr int kMmaWG = 3;               // warps 0-11: three MMA warpgroups (rows 64w..64w+63 of the row tile) + epilogue
+constexpr int kMmaThreads = kMmaWG * 128;
+constexpr int kProdWarp = kMmaWG * 4;   // warp 12: flag poll + TMA producer
+constexpr int kGateWarp0 = kProdWarp + 1;   // warps 13-20: gates
+constexpr int kGateThreads = 256;
 constexpr int kThreads = kGateWarp0 * 32 + kGateThreads;
+constexpr int kMaxRows = 64 * kMmaWG;
 constexpr int kMaxNS = 8;
-constexpr int kMaxWords = 9;            // K chunks x gate groups summed per gate element
-constexpr int kMaxDps = 14;             // units finished per CTA and step (4 gate elements per epilogue thread at n = 32)
+constexpr int kMaxWords = 12;           // K chunks x gate groups summed per gate element
+constexpr int kMaxDps = 16;             // units finished per CTA and step
+constexpr int kMaxCtasPerDir = 74;      // bound of the device-independent scratch sizes
 constexpr long long kSpinLimit = 2000000000LL;
 constexpr int kCtrStride = 32;          // counters live in separate 128-byte lines
 
@@ -70,7 +70,7 @@ struct EncTc {
     unsigned* bar;              // [32 * (dir*NT + tile)]: arrivals of the tile's CTAs (zero-initialised)
     unsigned long long* dbg;    // optional phase stamps of CTA 0 (NULL = off)
     int Tx, n, D, Kp;
-    int NT, S, dpc, dps, Kc, nkbA, NS;
+    int NT, S, dpc, dps, Kc, nkbA, NS, nwg;   // nwg: warpgroups holding rows of the tile (k-block = nwg * 8 KB of shared memory)
 };
 
 // bounded waits: a protocol error becomes a trap (context error), never a hung GPU
@@ -90,12 +90,6 @@ __device__ __forceinline__ void mbar_wait_b(uint64_t* bar, uint32_t parity) {
 __device__ __forceinline__ void flag_arrive(unsigned* ctr) {
     asm volatile("red.release.gpu.global.add.u32 [%0], 1;" ::"l"(ctr) : "memory");
 }
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, uint32_t (&r)[8]) {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-                 : "r"(taddr)
-                 : "memory");
-}
 // K-partial exchange words: {fp32 value, step tag} in ONE naturally aligned 64-bit word (single-copy atomic), written with
 // a relaxed gpu-scope store and polled with relaxed gpu-scope loads: no fence, no counter, one L2 round trip.
 __device__ __forceinline__ void st_word(unsigned long long* p, float v, uint32_t tag) {
@@ -109,27 +103,37 @@ __device__ __forceinline__ unsigned long long ld_word(const unsigned long long* 
 }
 
 // shared-memory byte offset of element (row m, k) inside a K-major SWIZZLE_128B operand made of 32-deep k-blocks of
-// 128 rows x 128 B (8-row groups 1024 B apart, 16-byte chunks XOR (m & 7))
-__device__ __forceinline__ uint32_t a_off(int m, int k) {
+// kb_bytes (rows of 128 B, 8-row groups 1024 B apart, 16-byte chunks XOR (m & 7))
+__device__ __forceinline__ uint32_t a_off(int m, int k, uint32_t kb_bytes) {
     const int kb = k >> 5, kk = k & 31;
-    return (uint32_t)kb * 16384u + (uint32_t)(m >> 3) * 1024u + (uint32_t)(m & 7) * 128u +
-           (uint32_t)(((kk >> 2) ^ (m & 7)) << 4) + (uint32_t)((kk & 3) << 2);
+    return (uint32_t)kb * kb_bytes + (uint32_t)m * 128u + (uint32_t)(((kk >> 2) ^ (m & 7)) << 4) + (uint32_t)((kk & 3) << 2);
+}
+
+template <int BN>
+__device__ __forceinline__ void mma_ss(float (&d)[BN / 2], uint64_t da, uint64_t db) {
+    if constexpr (BN == 32) wgmma_ss_n32(d, da, db);
+    else wgmma_ss_n64(d, da, db);
+}
+template <int BN>
+__device__ __forceinline__ void mma_rs(float (&d)[BN / 2], const uint32_t (&a)[4], uint64_t db) {
+    if constexpr (BN == 32) wgmma_rs_n32(d, a, db);
+    else wgmma_rs_n64(d, a, db);
 }
 
 template <int BN, bool BWD>
 __global__ void __launch_bounds__(kThreads, 1) enc_tc_kernel(const __grid_constant__ EncTc a) {
     constexpr uint32_t kStage = 2u * BN * 128u;             // [B_raw BN rows x 128 B | B_lo]
-    constexpr uint32_t kAcc2 = 4u * BN, kLoCol = 5u * BN;   // TMEM columns: acc0 [0,2BN) acc1 [2BN,4BN) lo.hi [4BN,5BN) A_lo [5BN, ..)
     constexpr int EPT = (kMaxDps * BN + kGateThreads - 1) / kGateThreads;   // gate elements per gate thread
     constexpr int NG = BWD ? 1 : 3;                         // gate column groups inside a row tile
+    constexpr int R = BN / 2;                               // accumulator registers per MMA thread
 
     extern __shared__ __align__(1024) unsigned char smem[];
     __shared__ __align__(8) uint64_t full[kMaxNS];
-    __shared__ __align__(8) uint64_t done[kMaxNS / 2];
-    __shared__ __align__(8) uint64_t accum_bar;
-    __shared__ uint32_t tmem_slot;
+    __shared__ __align__(8) uint64_t empty[kMaxNS];
 
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    // the warp index as a shuffled (provably warp-uniform) value: role branches on it are not divergent for the compiler,
+    // which would otherwise serialize the wgmma instructions inside them
+    const int tid = threadIdx.x, warp = __shfl_sync(0xffffffffu, tid >> 5, 0), lane = tid & 31;
     const int D = a.D, n = a.n, Tx = a.Tx, D3 = 3 * a.D, C = 2 * a.D;
     const int S = a.S, NT = a.NT, dpc = a.dpc, dps = a.dps;
     const int dir = blockIdx.x / (NT * S);
@@ -143,28 +147,22 @@ __global__ void __launch_bounds__(kThreads, 1) enc_tc_kernel(const __grid_consta
     const int klen = max(0, kend - kbeg);
     const int nkb = (klen + 31) >> 5;
     const int NS = a.NS;
+    const uint32_t kb_bytes = (uint32_t)a.nwg * 8192u;
 
-    const uint32_t sA = smem_u32(smem);
-    if (sA & 1023u) __trap();                                // the UMMA / TMA swizzle atoms need 1024-byte alignment
-    const uint32_t sRing = sA + (uint32_t)a.nkbA * 16384u;
+    const uint32_t sA = (smem_u32(smem) + 1023u) & ~1023u;   // the wgmma / TMA swizzle atoms need 1024-byte alignment
+    const uint32_t sRing = sA + (uint32_t)a.nkbA * kb_bytes;
 
-    // ------------------------------------------------------------------ prologue: weights -> shared (raw) + TMEM (lo)
+    // ------------------------------------------------------------------ prologue: weights -> shared (raw)
     {
-        const uint32_t words = (uint32_t)a.nkbA * 4096u;
+        const uint32_t words = (uint32_t)a.nkbA * kb_bytes / 4u;
         for (uint32_t i = tid; i < words / 4; i += kThreads)
             asm volatile("st.shared.v4.f32 [%0], {%1,%1,%1,%1};" ::"r"(sA + i * 16u), "f"(0.f) : "memory");
     }
     if (tid == 0) {
         asm volatile("prefetch.tensormap [%0];" ::"l"(&a.map_raw[dir]) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&a.map_lo[dir]) : "memory");
-        for (int s = 0; s < NS / 2; ++s) mbar_init(&full[s], 1);      // one per pair of ring stages
-        for (int s = 0; s < NS / 2; ++s) mbar_init(&done[s], 2);      // both MMA issuers commit
-        mbar_init(&accum_bar, 2);
+        for (int s = 0; s < NS; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], kMmaThreads / 32); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 0) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_slot)), "r"(512) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
     }
     __syncthreads();
     {
@@ -176,61 +174,31 @@ __global__ void __launch_bounds__(kThreads, 1) enc_tc_kernel(const __grid_consta
                 const int kl = e / rows, mm = e - kl * rows;
                 const int g = mm / nd, dl = mm - g * nd;
                 const float v = __ldg(W + (long long)(kbeg + kl) * D3 + g * D + d0 + dl);
-                asm volatile("st.shared.f32 [%0], %1;" ::"r"(sA + a_off(g * dpc + dl, kl)), "f"(v) : "memory");
+                asm volatile("st.shared.f32 [%0], %1;" ::"r"(sA + a_off(g * dpc + dl, kl, kb_bytes)), "f"(v) : "memory");
             }
         } else {                                             // rows = units d0 + m of d h_{t-1}, k = gate column: [U|Ux]^T
             const int total = nd * klen;
             for (int e = tid; e < total; e += kThreads) {
                 const int m = e / klen, kl = e - m * klen;
                 const float v = __ldg(W + (long long)(d0 + m) * D3 + kbeg + kl);
-                asm volatile("st.shared.f32 [%0], %1;" ::"r"(sA + a_off(m, kl)), "f"(v) : "memory");
+                asm volatile("st.shared.f32 [%0], %1;" ::"r"(sA + a_off(m, kl, kb_bytes)), "f"(v) : "memory");
             }
         }
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem = tmem_slot;
-    if (warp < 4) {
-        const int m = 32 * warp + lane;
-        for (int kb = 0; kb < a.nkbA; ++kb) {
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                uint32_t lo[16];
-#pragma unroll
-                for (int cch = 0; cch < 4; ++cch) {
-                    float4 v;
-                    const uint32_t addr = sA + (uint32_t)kb * 16384u + (uint32_t)(m >> 3) * 1024u + (uint32_t)(m & 7) * 128u +
-                                          (uint32_t)((((4 * h + cch) ^ (m & 7))) << 4);
-                    asm volatile("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr));
-                    lo[4 * cch] = __float_as_uint(resid(v.x)); lo[4 * cch + 1] = __float_as_uint(resid(v.y));
-                    lo[4 * cch + 2] = __float_as_uint(resid(v.z)); lo[4 * cch + 3] = __float_as_uint(resid(v.w));
-                }
-                tmem_st16(tmem + ((uint32_t)(32 * warp) << 16) + kLoCol + (uint32_t)(kb * 32 + 16 * h), lo);
-            }
-        }
-        asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
     }
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");      // the raw tiles were written by generic stores
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
 
     unsigned* tctr = a.bar + (dir * NT + tile) * kCtrStride;      // arrivals of this row tile's gate warps (S * 8 per step)
     const bool stamp = a.dbg != nullptr && blockIdx.x == 0;
 #define ENC_STAMP(i) do { a.dbg[i] = gtimer(); a.dbg[32 + (i)] = (unsigned long long)clock64(); } while (0)
 
-    // Ring protocol.  A tcgen05.commit costs the issuing thread ~130 cycles (an MMA 48.6), so stages are released in
-    // PAIRS of k-blocks and only when the pair's stages are needed again within the same time step: at the start of a
-    // step every stage is free by construction (the flag this CTA waits for is raised after its own epilogue, i.e. after
-    // accum_bar, which covers every MMA of the previous step).
-    const int NP = NS >> 1;                                  // pair slots of the ring
-    const int npair = (nkb + 1) >> 1;
-    if (warp == 4) {
+    // Ring protocol: k-block j of the CTA's whole run (all steps) uses stage j % NS; the producer refills a stage once all
+    // twelve MMA warps have arrived on its `empty` barrier (after the wgmmas that read it completed).
+    if (warp == kProdWarp) {
         // ============================================================ flag poll + TMA producer
         // Dependencies are tracked per ROW TILE (S arrivals per step each): this CTA's operand columns [kbeg, kcov) are
-        // produced by a few tiles only (9-10 of 24 forward, all 8 backward), so it does not wait for the slowest CTA of
-        // the whole direction.  Lane l polls the counter of tile l; the warp proceeds when every needed tile is complete.
+        // produced by a few tiles only, so it does not wait for the slowest CTA of the whole direction.  Lane l polls the
+        // counter of tile l; the warp proceeds when every needed tile is complete.
         const int kcov = min(Ktot, kbeg + 32 * nkb);
         bool need = false;
         if (lane < NT) {
@@ -238,7 +206,7 @@ __global__ void __launch_bounds__(kThreads, 1) enc_tc_kernel(const __grid_consta
             for (int g = 0; g < (BWD ? 3 : 1); ++g) need = need || (g * D + u0 < kcov && g * D + u1 > kbeg);
         }
         const unsigned* pctr = a.bar + (dir * NT + lane) * kCtrStride;
-        uint32_t dpar = 0;                                   // parity bit per pair slot: next phase of done[slot] to wait for
+        uint32_t it = 0;
         for (int s = 1; s < Tx; ++s) {
             {
                 const unsigned target = (unsigned)(S * (kGateThreads / 32) * s);
@@ -260,126 +228,95 @@ __global__ void __launch_bounds__(kThreads, 1) enc_tc_kernel(const __grid_consta
                 const int brow = BWD ? (dir == 0 ? Tx - s : s - 1) : (dir == 0 ? s - 1 : Tx - s);
                 asm volatile("fence.proxy.async;" ::: "memory");      // the operand was written by generic stores of other SMs
                 if (stamp && s == 8) ENC_STAMP(0);
-                for (int pr = 0; pr < npair; ++pr) {
-                    const int slot = pr % NP;
-                    if (pr >= NP) {
-                        mbar_wait_b(&done[slot], (dpar >> slot) & 1u);
-                        dpar ^= 1u << slot;
-                    }
-                    const int nb = min(2, nkb - 2 * pr);             // k-blocks of this pair (the last pair may be single)
-                    mbar_expect_tx(&full[slot], (uint32_t)nb * kStage);
-#pragma unroll
-                    for (int q = 0; q < 2; ++q) {
-                        if (q < nb) {
-                            const int kb = 2 * pr + q;
-                            const uint32_t dst = sRing + (uint32_t)(2 * slot + q) * kStage;
-                            tma_load_3d(dst, &a.map_raw[dir], &full[slot], kbeg + 32 * kb, 0, brow);
-                            tma_load_3d(dst + BN * 128u, &a.map_lo[dir], &full[slot], kbeg + 32 * kb, 0, (s - 1) & 1);
-                        }
-                    }
+                for (int kb = 0; kb < nkb; ++kb, ++it) {
+                    const uint32_t slot = it % (uint32_t)NS;
+                    if (it >= (uint32_t)NS) mbar_wait_b(&empty[slot], ((it / (uint32_t)NS) - 1u) & 1u);
+                    mbar_expect_tx(&full[slot], kStage);
+                    const uint32_t dst = sRing + slot * kStage;
+                    tma_load_3d(dst, &a.map_raw[dir], &full[slot], kbeg + 32 * kb, 0, brow);
+                    tma_load_3d(dst + BN * 128u, &a.map_lo[dir], &full[slot], kbeg + 32 * kb, 0, (s - 1) & 1);
                 }
             }
             __syncwarp();
         }
-    } else if (warp == 5 || warp == 6) {
-        // ============================================================ MMA issuers
-        // Straight-line issue code: a single thread executes dependent scalar instructions at ~10 cycles each, so every
-        // predicate / address computation between two MMAs shows up directly in the step time (the first version of this
-        // loop spent 275 cycles per k-step on bookkeeping where the two MMAs need 97).  Hence: fixed 4 k-steps per block
-        // (the weight tile is zero-padded, the operand tile zero-filled by TMA), the first block of a step peeled (its MMAs
-        // overwrite the accumulators), descriptors advanced by constant increments, and TWO issuing threads: warp 5 issues
-        // the N-stacked A_raw(shared) x [B_raw|B_lo] products into the two rotating accumulators, warp 6 the
-        // A_lo(tensor memory) x B_raw products into the third.  Each commits its own MMAs (barrier counts of 2).
-        if (lane == 0) {
-            const uint32_t idesc_base = (1u << 4) | (2u << 7) | (2u << 10) | ((128u >> 4) << 24);
-            const uint32_t idesc1 = idesc_base | ((uint32_t)(BN >> 3) << 17);
-            const uint32_t idesc2 = idesc_base | ((uint32_t)((2 * BN) >> 3) << 17);
-            const uint32_t acc0 = tmem, acc1 = tmem + 2u * BN, acc2 = tmem + kAcc2;
-            const uint64_t adesc0 = desc_kmajor(sA), bdesc0 = desc_kmajor(sRing);
-            const int ncommit = max(0, npair - NP);          // pairs whose stages are reused within a step
-            const int nkb_l = nkb, Tx_l = Tx;
-            const bool ss = warp == 5;
-            uint32_t fpar = 0;                               // parity bit per pair slot: next phase of full[slot]
-            const int npair_l = npair, NP_l = NP;
-            const bool odd = (nkb_l & 1) != 0;               // the last pair holds a single k-block
-            for (int s = 1; s < Tx_l; ++s) {
-                uint64_t adesc = adesc0;
-                uint32_t alo = tmem + kLoCol;
-                int slot = 0;
-                // one full barrier per PAIR of k-blocks: the per-block bookkeeping of this single thread (wait, parity,
-                // descriptor arithmetic: ~10 cycles per dependent scalar instruction) costs as much as the MMAs themselves
-#define ENC_MMA_4(FIRST, AD, AL, BD)                                                                                 \
-    if (ss) {                                                                                                        \
-        if (ENC_TC_DBG != 2) {                                                                                       \
-            umma_tf32(acc0, (AD), (BD), idesc2, (FIRST) ? 0u : 1u);                                                  \
-            umma_tf32(acc1, (AD) + 2, (BD) + 2, idesc2, (FIRST) ? 0u : 1u);                                          \
-            umma_tf32(acc0, (AD) + 4, (BD) + 4, idesc2, 1u);                                                         \
-            umma_tf32(acc1, (AD) + 6, (BD) + 6, idesc2, 1u);                                                         \
-        }                                                                                                            \
-    } else if (ENC_TC_DBG != 3) {                                                                                    \
-        umma_tf32_ts(acc2, (AL), (BD), idesc1, (FIRST) ? 0u : 1u);                                                   \
-        umma_tf32_ts(acc2, (AL) + 8, (BD) + 2, idesc1, 1u);                                                          \
-        umma_tf32_ts(acc2, (AL) + 16, (BD) + 4, idesc1, 1u);                                                         \
-        umma_tf32_ts(acc2, (AL) + 24, (BD) + 6, idesc1, 1u);                                                         \
-    }
-                for (int pr = 0; pr < npair_l; ++pr) {
-                    mbar_wait_b(&full[slot], (fpar >> slot) & 1u);
-                    fpar ^= 1u << slot;
-                    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                    const uint64_t bdesc = bdesc0 + (uint64_t)((uint32_t)slot * (2u * (kStage >> 4)));
-                    if (pr == 0) {
-                        ENC_MMA_4(true, adesc, alo, bdesc)
-                        if (stamp && ss && s == 8) ENC_STAMP(1);
-                    } else {
-                        ENC_MMA_4(false, adesc, alo, bdesc)
-                    }
-                    if (!(odd && pr == npair_l - 1)) { ENC_MMA_4(false, adesc + 1024, alo + 32, bdesc + (kStage >> 4)) }
-                    if (ENC_TC_DBG != 1) adesc += 2048;
-                    alo += 64;
-                    if (pr < ncommit) umma_commit(&done[slot]);
-                    slot = (slot + 1 == NP_l) ? 0 : slot + 1;
-                }
-                umma_commit(&accum_bar);
-                if (stamp && ss && s == 8) ENC_STAMP(2);
-            }
+    } else if (warp < kProdWarp) {
+        // ============================================================ MMA warpgroups: K partials of this CTA's chunk
+        const int wg = warp >> 2;
+        const bool active = wg < a.nwg;                      // warpgroup-uniform: rows 64wg.. hold weights
+        const int r0 = 64 * wg + 16 * (warp & 3) + (lane >> 2);       // fragment rows r0, r0 + 8
+        const int q = lane & 3;
+        int g_row[2], dl_row[2];
+        bool row_ok[2];
+        unsigned long long* slab_w[2];
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int mrow = r0 + 8 * h;
+            g_row[h] = BWD ? 0 : mrow / dpc;
+            dl_row[h] = mrow - g_row[h] * dpc;
+            row_ok[h] = g_row[h] < NG && dl_row[h] < nd;
+            slab_w[h] = a.slab + (long long)(dir * NT + tile) * S * NG * BN * dpc +
+                        (long long)((crank * NG + g_row[h]) * BN) * dpc + dl_row[h];      // + b*dpc
         }
-    } else if (warp < 4) {
-        // ============================================================ TMEM warps: accumulators -> K-partial words of this CTA's chunk
-        const int mrow = 32 * warp + lane;
-        const int g_row = BWD ? 0 : mrow / dpc;
-        const int dl_row = mrow - g_row * dpc;
-        const bool row_ok = g_row < NG && dl_row < nd;
-        unsigned long long* slab_w = a.slab + (long long)(dir * NT + tile) * S * NG * BN * dpc +
-                                     (long long)((crank * NG + g_row) * BN) * dpc + dl_row;      // + b*dpc
+        const uint32_t a_row0 = sA + (uint32_t)r0 * 128u, a_row1 = a_row0 + 1024u;  // rows r0 and r0 + 8: same (m & 7)
+        const uint32_t sw = (uint32_t)(r0 & 7);
+        const uint64_t adesc0 = desc_sw128(sA + (uint32_t)wg * 8192u);
+        const uint64_t bdesc0 = desc_sw128(sRing);
+        uint32_t it = 0;
         for (int s = 1; s < Tx; ++s) {
-            {
-                mbar_wait_b(&accum_bar, (uint32_t)((s - 1) & 1));
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                if (stamp && s == 8 && tid == 0) ENC_STAMP(3);
+            float acc_hh[R], acc_x[R];
 #pragma unroll
-                for (int c0 = 0; c0 < BN; c0 += 8) {
-                    uint32_t t0[8], t1[8], t2[8], t3[8], t4[8];
-                    const uint32_t ta = tmem + ((uint32_t)(32 * warp) << 16) + (uint32_t)c0;
-                    tmem_ld8(ta, t0);                     // acc0 hi.hi
-                    tmem_ld8(ta + 2 * BN, t1);            // acc1 hi.hi
-                    tmem_ld8(ta + BN, t2);                // acc0 hi.lo
-                    tmem_ld8(ta + 3 * BN, t3);            // acc1 hi.lo
-                    tmem_ld8(ta + kAcc2, t4);             // lo.hi
-                    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-                    if (row_ok) {
+            for (int i = 0; i < R; ++i) { acc_hh[i] = 0.f; acc_x[i] = 0.f; }
+            for (int kb = 0; kb < nkb; ++kb, ++it) {
+                const uint32_t slot = it % (uint32_t)NS;
+                // residual A fragments of the 4 k-steps (rows r0 / r0+8, k = 8kk + q and 8kk + q + 4)
+                uint32_t alo[4][4];
 #pragma unroll
-                        for (int q = 0; q < 8; ++q)
-                            st_word(slab_w + (long long)(c0 + q) * dpc,
-                                    (__uint_as_float(t0[q]) + __uint_as_float(t1[q])) +
-                                        ((__uint_as_float(t2[q]) + __uint_as_float(t3[q])) + __uint_as_float(t4[q])),
-                                    (uint32_t)s);
-                    }
+                for (int kk = 0; kk < 4; ++kk) {
+                    const uint32_t c0 = (((uint32_t)(2 * kk) ^ sw) << 4) + (uint32_t)(q << 2);
+                    const uint32_t c1 = (((uint32_t)(2 * kk + 1) ^ sw) << 4) + (uint32_t)(q << 2);
+                    const uint32_t kbo = (uint32_t)kb * kb_bytes;
+                    float v0, v1, v2, v3;
+                    asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v0) : "r"(a_row0 + kbo + c0));
+                    asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v1) : "r"(a_row1 + kbo + c0));
+                    asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v2) : "r"(a_row0 + kbo + c1));
+                    asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v3) : "r"(a_row1 + kbo + c1));
+                    alo[kk][0] = __float_as_uint(resid(v0)); alo[kk][1] = __float_as_uint(resid(v1));
+                    alo[kk][2] = __float_as_uint(resid(v2)); alo[kk][3] = __float_as_uint(resid(v3));
                 }
-                asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-                if (stamp && s == 8 && tid == 0) ENC_STAMP(6);
-                // the peers' partials are written at about the same time as ours: only now do the gate warps start polling
-                asm volatile("bar.arrive 2, %0;" ::"r"(128 + kGateThreads) : "memory");
+                mbar_wait_b(&full[slot], (it / (uint32_t)NS) & 1u);
+                if (active) {
+                    const uint64_t ad = adesc0 + (uint64_t)((kb * kb_bytes) >> 4);
+                    const uint64_t braw = bdesc0 + (uint64_t)((slot * kStage) >> 4), blo = braw + (uint64_t)((BN * 128u) >> 4);
+                    wgmma_fence();
+#pragma unroll
+                    for (int kk = 0; kk < 4; ++kk) {
+                        mma_ss<BN>(acc_hh, ad + 2 * kk, braw + 2 * kk);
+                        mma_ss<BN>(acc_x, ad + 2 * kk, blo + 2 * kk);
+                        mma_rs<BN>(acc_x, alo[kk], braw + 2 * kk);
+                    }
+                    wgmma_commit();
+                    wgmma_wait<0>();
+                    reg_fence(acc_hh); reg_fence(acc_x);
+                }
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&empty[slot]);
             }
+            if (stamp && s == 8 && tid == 0) ENC_STAMP(3);
+            // fragment i of this thread: row r0 + 8*((i>>1)&1), batch column 8*(i>>2) + 2q + (i&1)
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                if (!row_ok[h]) continue;
+#pragma unroll
+                for (int j = 0; j < BN / 8; ++j)
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+                        const int i = 4 * j + 2 * h + e;
+                        st_word(slab_w[h] + (long long)(8 * j + 2 * q + e) * dpc, acc_hh[i] + acc_x[i], (uint32_t)s);
+                    }
+            }
+            if (stamp && s == 8 && tid == 0) ENC_STAMP(6);
+            // the peers' partials are written at about the same time as ours: only now do the gate warps start polling
+            asm volatile("bar.arrive 2, %0;" ::"r"(kMmaThreads + kGateThreads) : "memory");
         }
     } else {
         // ============================================================ gate warps: K partials of the tile -> gates of this CTA's units
@@ -481,7 +418,7 @@ __global__ void __launch_bounds__(kThreads, 1) enc_tc_kernel(const __grid_consta
                 }
             };
             if (s > 0) {
-                named_bar_sync(2, 128 + kGateThreads);       // (256 pollers spinning through the whole product would starve the TMEM warps' stores)
+                named_bar_sync(2, kMmaThreads + kGateThreads);       // (256 pollers spinning through the whole product would starve the MMA warps' stores)
 #pragma unroll
                 for (int i0 = 0; i0 < EPT; i0 += 2) {
                     unsigned long long w[2][kMaxWords];
@@ -571,10 +508,6 @@ __global__ void __launch_bounds__(kThreads, 1) enc_tc_kernel(const __grid_consta
                 if (ev[i]) a.ctxsum[(long long)eb[i] * C + dir * D + dbase + ed[i]] = csum[i];
         }
     }
-    __syncwarp();
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(512) : "memory");
 }
 
 // ------------------------------------------------------------------ host side
@@ -604,60 +537,53 @@ int make_map(const float* ptr, long long inner, long long rows, long long outer,
 
 struct TcPlan {
     bool ok;
-    int BN, NT, S, NG, dpc, dps, Kc, nkbA, NS, Ktot;
+    int BN, NT, S, NG, dpc, dps, Kc, nkbA, NS, Ktot, nwg;
     size_t smem;
     long long slab_floats, lo_floats, counter_ints;
 };
 
-// pass 0: rows = 3 gate columns x dpc units (dpc <= 42), K = D in S = 3 chunks;
-// pass 1: rows = dpc units (<= 128), K = 3D in S chunks of <= 352
+// Row tiles of <= 192 rows (forward: 3 gate columns x dpc units; backward: dpc units), K cut into S chunks.  Among the S whose
+// weight tile fits next to a ring of at least two stages in shared memory, the one with the fewest k-blocks per CTA wins
+// (the k-blocks of a step are a serial chain of MMAs, the exchange words grow only linearly), ties to the smaller S.
 TcPlan plan(const nats_ctx* ctx, int n, int D, int pass) {
     TcPlan p;
     memset(&p, 0, sizeof(p));
     if (g_enc == nullptr || n < 1 || n > 64 || D < 96 || (D & 3)) return p;
     p.BN = n <= 32 ? 32 : 64;
-    const int per_dir = ctx->num_sms / 2;
-    const int max_cols = 512 - 5 * p.BN;                     // tensor memory left for the resident A_lo
-    const size_t lim = (size_t)ctx->max_smem_optin - g_static_smem;
+    const int per_dir = min(ctx->num_sms / 2, kMaxCtasPerDir);
+    const size_t lim = (size_t)ctx->max_smem_optin - g_static_smem - 1024;     // 1 KB: alignment of the dynamic base
     const size_t stage = (size_t)2 * p.BN * 128;
-    int max_kb = max_cols / 32;
-    if ((size_t)max_kb * 16384 + 2 * stage > lim) max_kb = (int)((lim - 2 * stage) / 16384);
-    if (max_kb < 1) return p;
-    if (pass == 0) {
-        p.NG = 3; p.Ktot = D; p.S = 3;
-        p.NT = per_dir / p.S;
-        if (p.NT < 1) return p;
-        p.dpc = (D + p.NT - 1) / p.NT;
-        if (p.dpc > 42) return p;
-    } else {
-        p.NG = 1; p.Ktot = 3 * D;
-        p.S = (p.Ktot + max_kb * 32 - 1) / (max_kb * 32);
-        if (p.S < 2) p.S = 2;
-        p.NT = per_dir / p.S;
-        if (p.NT < 1) return p;
-        p.dpc = (D + p.NT - 1) / p.NT;
-        if (p.dpc > 128) return p;
+    p.NG = pass == 0 ? 3 : 1;
+    p.Ktot = pass == 0 ? D : 3 * D;
+    TcPlan best = p;
+    for (int S = 2; S <= kMaxWords / p.NG; ++S) {
+        const int NT0 = per_dir / S;
+        if (NT0 < 1) break;
+        const int dpc = (D + NT0 - 1) / NT0;
+        const int NT = (D + dpc - 1) / dpc;
+        const int rows = p.NG * dpc;
+        if (rows > kMaxRows || NT > 32) continue;
+        const int dps = (dpc + S - 1) / S;
+        if (dps > kMaxDps) continue;
+        const int Kc = (((p.Ktot + S - 1) / S + 31) / 32) * 32;
+        if (p.Ktot - Kc * (S - 1) < 8) continue;                  // every CTA owns at least one k-step
+        const int nwg = (rows + 63) / 64;
+        const size_t fixed = (size_t)(Kc / 32) * nwg * 8192;
+        if (fixed + 2 * stage > lim) continue;
+        if (best.ok && Kc / 32 >= best.nkbA) continue;
+        p.S = S; p.NT = NT; p.dpc = dpc; p.dps = dps; p.Kc = Kc; p.nkbA = Kc / 32; p.nwg = nwg;
+        p.NS = (int)((lim - fixed) / stage);
+        if (p.NS > kMaxNS) p.NS = kMaxNS;
+        if (p.NS > p.nkbA) p.NS = max(2, p.nkbA);
+        p.smem = fixed + (size_t)p.NS * stage + 1024;
+        const long long Kp = (p.Ktot + 3) / 4 * 4;
+        p.lo_floats = (4LL * n * Kp + 3) / 4 * 4;
+        p.slab_floats = 2LL * (2LL * p.NT * p.S * p.NG * p.BN * p.dpc);      // 64-bit words
+        p.counter_ints = 2LL * p.NT * kCtrStride;
+        p.ok = true;
+        best = p;
     }
-    p.NT = (D + p.dpc - 1) / p.dpc;
-    p.dps = (p.dpc + p.S - 1) / p.S;
-    if (p.dps > kMaxDps) return p;
-    p.Kc = (((p.Ktot + p.S - 1) / p.S + 31) / 32) * 32;
-    if (p.Ktot - p.Kc * (p.S - 1) < 16) return p;            // every CTA owns >= 2 k-steps (both rotating accumulators get written)
-    p.nkbA = p.Kc / 32;
-    if (p.nkbA > max_kb) return p;
-    const size_t fixed = (size_t)p.nkbA * 16384;
-    p.NS = (int)((lim - fixed) / stage) & ~1;                // pairs of stages
-    if (p.NS > kMaxNS) p.NS = kMaxNS;
-    if (p.NS > ((p.nkbA + 1) & ~1)) p.NS = (p.nkbA + 1) & ~1;
-    if (p.NS < 2) return p;
-    p.smem = fixed + (size_t)p.NS * stage;
-    const long long Kp = (p.Ktot + 3) / 4 * 4;
-    p.lo_floats = (4LL * n * Kp + 3) / 4 * 4;
-    if (p.S * p.NG > kMaxWords || p.NT > 32) return p;
-    p.slab_floats = 2LL * (2LL * p.NT * p.S * p.NG * p.BN * p.dpc);      // 64-bit words
-    p.counter_ints = 2LL * p.NT * kCtrStride;
-    p.ok = true;
-    return p;
+    return best;
 }
 
 template <int BN, bool BWD>
@@ -704,10 +630,10 @@ bool enc_tc_eligible(const nats_ctx* ctx, int n, int D, int pass) {
 }
 
 // upper bounds that do not depend on the device (workspace carving happens without a context):
-// residual side buffer 4*n*(3D+4) floats + K-partial words: 2 directions x <= 74 CTAs x 128 rows x BN batch columns
+// residual side buffer 4*n*(3D+4) floats + K-partial words: 2 directions x <= 74 CTAs x 192 rows x BN batch columns
 long long enc_tc_scratch_floats(int n, int D) {
     const long long BN = n <= 32 ? 32 : 64;
-    return 4LL * n * (3LL * D + 4) + 2LL * (2LL * 74 * 128 * BN) + 64;
+    return 4LL * n * (3LL * D + 4) + 2LL * (2LL * kMaxCtasPerDir * kMaxRows * BN) + 64;
 }
 long long enc_tc_counter_ints() { return 2LL * 32 * kCtrStride + 64; }
 
@@ -727,7 +653,7 @@ int enc_tc_fwd(const nats_ctx* ctx, cudaStream_t st, const EncTcFwdArgs& g) {
     }
     a.mask = g.mask; a.cc = g.cc; a.lo = g.scratch; a.slab = reinterpret_cast<unsigned long long*>(g.scratch + pl.lo_floats); a.ctxsum = g.ctxsum; a.bar = g.bar; a.dbg = g.dbg;
     a.Tx = g.Tx; a.n = n; a.D = D; a.Kp = Kp;
-    a.NT = pl.NT; a.S = pl.S; a.dpc = pl.dpc; a.dps = pl.dps; a.Kc = pl.Kc; a.nkbA = pl.nkbA; a.NS = pl.NS;
+    a.NT = pl.NT; a.S = pl.S; a.dpc = pl.dpc; a.dps = pl.dps; a.Kc = pl.Kc; a.nkbA = pl.nkbA; a.NS = pl.NS; a.nwg = pl.nwg;
     NATS_CUDA_OK(memset_async(st, g.bar, 0, (size_t)pl.counter_ints * sizeof(unsigned)));
     NATS_CUDA_OK(memset_async(st, g.scratch + pl.lo_floats, 0xff, (size_t)pl.slab_floats * sizeof(float)));     // no stale step tags
     ProfScope ps(st, K_ENC_PERSIST_FWD, 2.0 * 2 * g.Tx * (double)n * 3.0 * D * D, 4.0 * 2 * 3.0 * D * D);
@@ -754,7 +680,7 @@ int enc_tc_bwd(const nats_ctx* ctx, cudaStream_t st, const EncTcBwdArgs& g) {
     a.mask = g.mask; a.cc = const_cast<float*>(g.cc); a.dcc = g.dcc; a.mean_grad = g.mean_grad; a.coef = g.coef;
     a.lo = g.scratch; a.slab = reinterpret_cast<unsigned long long*>(g.scratch + pl.lo_floats); a.bar = g.bar; a.dbg = g.dbg;
     a.Tx = g.Tx; a.n = n; a.D = D; a.Kp = Kp;
-    a.NT = pl.NT; a.S = pl.S; a.dpc = pl.dpc; a.dps = pl.dps; a.Kc = pl.Kc; a.nkbA = pl.nkbA; a.NS = pl.NS;
+    a.NT = pl.NT; a.S = pl.S; a.dpc = pl.dpc; a.dps = pl.dps; a.Kc = pl.Kc; a.nkbA = pl.nkbA; a.NS = pl.NS; a.nwg = pl.nwg;
     NATS_CUDA_OK(memset_async(st, g.bar, 0, (size_t)pl.counter_ints * sizeof(unsigned)));
     NATS_CUDA_OK(memset_async(st, g.scratch + pl.lo_floats, 0xff, (size_t)pl.slab_floats * sizeof(float)));     // no stale step tags
     ProfScope ps(st, K_ENC_PERSIST_BWD, 2.0 * 2 * g.Tx * (double)n * 3.0 * D * D, 4.0 * 2 * 3.0 * D * D);

@@ -261,7 +261,7 @@ __global__ void reduce_splits_kernel(const float* __restrict__ part, int nsplit,
 
 }  // namespace
 
-static int g_use_tc = 2;      // 0: FFMA, 1: tcgen05 with software loaders, 2: tcgen05 fed by TMA where possible
+static int g_use_tc = 2;      // 0: FFMA, 1: wgmma with software loaders, 2: wgmma fed by TMA where possible
 void gemm_set_tensor_cores(int on) { g_use_tc = on; }
 int gemm_get_tensor_cores() { return g_use_tc; }
 
@@ -320,7 +320,7 @@ int gemm_pick_split(const nats_ctx* ctx, int M, int N, int K, int groups) {
     int tiles;
     if (g_use_tc && (M >= 128 || N >= 128) && K >= 32) {
         const int a = M > N ? M : N, b = M > N ? N : M;      // 128-row side / N side of the tensor-core tile
-        const int bn = b <= 32 ? 32 : (b <= 64 ? 64 : 128);
+        const int bn = b <= 32 ? 32 : 64;
         tiles = cdiv(a, 128) * cdiv(b, bn);
     } else {
         const int bm = (M <= 32) ? 32 : 64, bn = (M <= 32) ? 128 : 64;
@@ -342,7 +342,7 @@ int reduce_splits(cudaStream_t st, const float* part, int nsplit, long long stri
     if (total == 0) return 0;
     const int block = 256;
     long long gl = (total + block - 1) / block;
-    if (gl > 148LL * 16) gl = 148LL * 16;
+    if (gl > 132LL * 16) gl = 132LL * 16;
     const int grid = (int)gl;
     ProfScope ps(st, K_REDUCE_SPLITS, 0.0, 4.0 * total * (nsplit + 1));
     NATS_CUDA_OK(launch_pdl(reduce_splits_kernel, dim3(grid), dim3(block), 0, st, part, nsplit, strideP, M, N, ldp, out, ldo, bias,
@@ -361,7 +361,7 @@ int gemm_auto(const nats_ctx* ctx, cudaStream_t st, GemmProblem p, bool transA, 
         const bool swapped = p.M < 128 && p.N > p.M;
         const int nb = swapped ? p.M : p.N, ma = swapped ? p.N : p.M;
         (void)a; (void)b;
-        const int bn = nb <= 32 ? 32 : (nb <= 64 ? 64 : 128);
+        const int bn = nb <= 32 ? 32 : 64;
         tiles = (long long)cdiv(ma, 128) * cdiv(nb, bn) * p.batch;
     } else {
         int bm, bn;
@@ -372,9 +372,10 @@ int gemm_auto(const nats_ctx* ctx, cudaStream_t st, GemmProblem p, bool transA, 
     }
     int splits = 1;
     if (tc && p.batch == 1 && tiles >= ctx->num_sms && p.K >= 4096 && scratch != nullptr) {
-        // deep products whose tile count is not a multiple of the SM count (d[U|Ux] of the encoder: 192 tiles of K = 12768
-        // on 148 SMs = 2 waves for 1.3 waves of work): pick the split-K factor that minimises waves x (k-blocks per CTA +
-        // fixed cost) + the slab reduction, in microseconds (0.75 us per 128x128x32 k-block of 3xTF32, measured)
+        // deep products whose tile count is not a multiple of the SM count (d[U|Ux] of the encoder at dim 1000: 376 tiles of
+        // K = 12768 on 132 SMs = 3 waves for 2.8 waves of work): pick the split-K factor that minimises waves x (k-blocks per
+        // CTA + fixed cost) + the slab reduction.  The costs are a model in microseconds (a 128x64x32 k-block of 3xTF32 against
+        // a fixed cost per CTA and the slab traffic), not measurements.
         double best = 1e30;
         for (int s2 = 1; s2 <= 4; ++s2) {
             if ((long long)s2 * p.M * p.N > scratch_floats) break;

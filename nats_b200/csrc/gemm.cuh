@@ -5,8 +5,7 @@
 // grouped (up to 4 problems per launch: e.g. both encoder directions), batched (strided), split-K
 // (each split writes its own partial slab, summed by the consumer kernel => deterministic, no atomics).
 //
-// v1 arithmetic is exact-fp32 FFMA (parity with the reference's floatX=float32 first); the tensor-core
-// (tcgen05, 3xTF32) variant of the large-K products is a later milestone -- see DESIGN.md.
+// Two engines: exact-fp32 FFMA tiles (gemm.cu) and fp32-grade 3xTF32 products on the tensor cores (tc_gemm.cu, wgmma).
 #pragma once
 #include "common.cuh"
 
@@ -26,7 +25,6 @@ struct GemmProblem {
     int kchunk;            // K range per split (multiple of 16)
     long long strideP;     // distance between split slabs of C
     int accumulate;        // C += result (only with splitk == 1)
-    int a_static, b_static; // operand is constant within the step (a weight matrix): PDL kernels may prefetch it early
 };
 
 constexpr int kGemmMaxGroup = 4;
@@ -60,14 +58,14 @@ inline void gemm_set_split(GemmProblem& p, int splits, long long strideP) {
     p.strideP = strideP;
 }
 
-// tensor-core path (tc_gemm.cu): same contract as gemm_launch, 3xTF32 on tcgen05
+// tensor-core path (tc_gemm.cu): same contract as gemm_launch, 3xTF32 on wgmma
 int tc_gemm_launch(cudaStream_t st, const GemmProblem* probs, int count, bool transA, bool transB);
 int tc_gemm_setup();
 // TMA-fed variant (tma_gemm.cu): needs 16-byte aligned operands with leading dimensions multiple of 4
 int tma_gemm_launch(cudaStream_t st, const GemmProblem* probs, int count, bool transA, bool transB);
 bool tma_gemm_eligible(const GemmProblem* probs, int count);
 int tma_gemm_setup();
-void gemm_set_tensor_cores(int on);     // 1 (default): GEMM-shaped work goes to tcgen05; 0: exact-fp32 FFMA kernels
+void gemm_set_tensor_cores(int on);     // 2 (default): tensor cores, TMA-fed where possible; 1: software loaders only; 0: FFMA
 int gemm_get_tensor_cores();
 
 // Low-level launch: all problems share transposition flags and tile configuration.

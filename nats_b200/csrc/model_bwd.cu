@@ -83,7 +83,6 @@ int train_decoder_bwd(const nats_ctx* ctx, cudaStream_t st, const nats_dims_t& d
             gemm_set_split(q[0], SA, spD);
             q[1] = gemm_problem(w.dG1x + r3, D3, params + o.W1cat, D3, w.part_a, C, B, C, D3);
             gemm_set_split(q[1], SB, spC);
-            q[0].b_static = q[1].b_static = 1;
             NATS_TRY(gemm_launch(st, q, 2, false, true, cfg));
         }
         {   // distraction + attention backward (nats.py:527-546, 569-570)
@@ -111,7 +110,6 @@ int train_decoder_bwd(const nats_ctx* ctx, cudaStream_t st, const nats_dims_t& d
         }
         {   // d h1 += d ps . W_att^T  (nats.py:527)
             GemmProblem q = gemm_problem(w.dps + rA, A, params + o.W_att, A, w.part_d, D, B, D, A);
-            q.b_static = 1;
             NATS_TRY(gemm_launch(st, &q, 1, false, true, cfg));
         }
         {   // GRU_2 backward (nats.py:505-518)
@@ -129,7 +127,6 @@ int train_decoder_bwd(const nats_ctx* ctx, cudaStream_t st, const nats_dims_t& d
         {   // d h_{t-1} through the GRU_2 recurrent product
             GemmProblem q = gemm_problem(w.dG2 + r3, D3, params + o.dec.Ucat, D3, w.part_c, D, B, D, D3);
             gemm_set_split(q, S4, spD);
-            q.b_static = 1;
             NATS_TRY(gemm_launch(st, &q, 1, false, true, cfg));
         }
     }
@@ -192,7 +189,7 @@ int train_encoder_bwd(const nats_ctx* ctx, cudaStream_t st, const nats_dims_t& d
     const int S = gemm_pick_split(ctx, B, D, D3, 2);
     const long long strideP = 2LL * B * D;
     const bool persistent = enc_tc_eligible(ctx, B, D, 1);
-    if (persistent) {      // the whole reverse recurrence of both directions in ONE persistent tcgen05 launch (enc_tc.cu)
+    if (persistent) {      // the whole reverse recurrence of both directions in ONE persistent wgmma launch (enc_tc.cu)
         EncTcBwdArgs pa;
         memset(&pa, 0, sizeof(pa));
         for (int dir = 0; dir < 2; ++dir) {
@@ -237,7 +234,6 @@ int train_encoder_bwd(const nats_ctx* ctx, cudaStream_t st, const nats_dims_t& d
                 q[dir] = gemm_problem(w.dGe[dir] + (long long)pos * B * D3, D3, params + o.enc[dir].Ucat, D3,
                                       w.part_a + (long long)dir * B * D, D, B, D, D3);
                 gemm_set_split(q[dir], S, strideP);
-                q[dir].b_static = 1;
             }
             NATS_TRY(gemm_launch(st, q, 2, false, true, cfg));
         }

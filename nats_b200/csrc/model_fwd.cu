@@ -5,7 +5,7 @@ namespace nats {
 
 // ------------------------------------------------------------------------------------------------
 // encoder: embedding gather, input projections of both directions (one grouped GEMM), then Tx recurrent
-// recurrent steps: ONE persistent tcgen05 launch for both directions (enc_tc.cu) or, for shapes it does not take,
+// recurrent steps: ONE persistent wgmma launch for both directions (enc_tc.cu) or, for shapes it does not take,
 // per-step launches where forward step s and backward step s share a grouped GEMM + a 2-group gate kernel.
 // States are written straight into the concatenated context [Tx, n, 2D] (nats.py:713 needs no copy), the
 // masked sum for ctx_mean (nats.py:717) is accumulated by the gate kernel.
@@ -29,7 +29,7 @@ int encoder_forward(const nats_ctx* ctx, cudaStream_t st, const nats_dims_t& d, 
     const int cfg = gemm_step_cfg(n);
     const long long strideP = 2LL * n * D3;
     if (enc_tc_eligible(ctx, n, D, 0) && e.enc_scratch != nullptr) {
-        // the whole recurrence of both directions in ONE persistent weight-stationary tcgen05 launch (enc_tc.cu)
+        // the whole recurrence of both directions in ONE persistent weight-stationary wgmma launch (enc_tc.cu)
         EncTcFwdArgs pa;
         memset(&pa, 0, sizeof(pa));
         for (int dir = 0; dir < 2; ++dir) {
@@ -52,7 +52,6 @@ int encoder_forward(const nats_ctx* ctx, cudaStream_t st, const nats_dims_t& d, 
                                     e.part_a + (long long)n * D3, D3, n, D3, D);
                 gemm_set_split(q[0], S, strideP);
                 gemm_set_split(q[1], S, strideP);
-                q[0].b_static = q[1].b_static = 1;
                 NATS_TRY(gemm_launch(st, q, 2, false, false, cfg));
             }
             GateFwd g[2];
@@ -104,7 +103,6 @@ int decoder_step_forward(const nats_ctx* ctx, cudaStream_t st, const nats_dims_t
     {   // GRU_2 recurrent product (nats.py:505, 512)
         GemmProblem q = gemm_problem(s.h_prev, D, params + o.dec.Ucat, D3, s.part_b, D3, n, D3, D);
         gemm_set_split(q, S1, sp3);
-        q.b_static = 1;
         NATS_TRY(gemm_launch(st, &q, 1, false, false, cfg));
         GateFwd g;
         memset(&g, 0, sizeof(g));
@@ -122,7 +120,6 @@ int decoder_step_forward(const nats_ctx* ctx, cudaStream_t st, const nats_dims_t
         gemm_set_split(q[0], S1, sp3);
         q[1] = gemm_problem(s.h1, D, params + o.W_att, A, s.part_d, A, n, A, D);
         gemm_set_split(q[1], S1, (long long)n * A);
-        q[0].b_static = q[1].b_static = 1;
         NATS_TRY(gemm_launch(st, q, 2, false, false, cfg));
     }
     {
@@ -145,7 +142,6 @@ int decoder_step_forward(const nats_ctx* ctx, cudaStream_t st, const nats_dims_t
     {   // GRU_1 (nats.py:551-565)
         GemmProblem q = gemm_problem(s.ctx_out, C, params + o.W1cat, D3, s.part_a, D3, n, D3, C);
         gemm_set_split(q, S2, sp3);
-        q.b_static = 1;
         NATS_TRY(gemm_launch(st, &q, 1, false, false, cfg));
         GateFwd g;
         memset(&g, 0, sizeof(g));

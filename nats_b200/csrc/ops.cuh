@@ -51,7 +51,7 @@ struct GateBwd {
 };
 int gru_gates_bwd(cudaStream_t st, const GateBwd* groups, int ngroups, int B, int D);
 
-// ------------------------------------------------------------------ persistent tcgen05 encoder recurrence (enc_tc.cu)
+// ------------------------------------------------------------------ persistent tensor-core encoder recurrence (enc_tc.cu)
 struct EncTcFwdArgs {
     const float* Ucat[2]; const float* xproj[2]; const float* mask; float* cc;
     float* r[2]; float* u[2]; float* c[2]; float* p[2];      // NULL = do not save
@@ -76,12 +76,10 @@ long long enc_tc_scratch_floats(int n, int D);     // upper bounds, independent 
 long long enc_tc_counter_ints();
 int enc_tc_fwd(const nats_ctx* ctx, cudaStream_t st, const EncTcFwdArgs& a);
 int enc_tc_bwd(const nats_ctx* ctx, cudaStream_t st, const EncTcBwdArgs& a);
-void gates_trace(int on);
-void attention_set_cc_keep(int mode);
-void tma_gemm_trace(int on);
-void tma_gemm_debug_mode(int mode);
 void tma_gemm_set_ts(int on);
 int tma_gemm_get_ts();
+void gates_trace(int on);
+void attention_set_cc_keep(int mode);
 
 // ------------------------------------------------------------------ small elementwise / reductions
 int tanh_inplace(cudaStream_t st, float* x, long long n);

@@ -6,7 +6,7 @@ namespace nats {
 
 namespace {
 
-constexpr int kRedBlocks = 148 * 4;
+constexpr int kRedBlocks = 132 * 4;
 
 __global__ void sumsq_stage1(const float* __restrict__ x, long long n, float* __restrict__ part) {
     __shared__ float red[32];

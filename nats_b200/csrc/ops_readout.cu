@@ -358,7 +358,7 @@ int softmax_sample_rows(cudaStream_t st, const float* logits, int rows, int V, f
     if (rows == 0) return 0;
     ProfScope ps(st, K_SOFTMAX_SAMPLE, 0.0, 16.0 * rows * V);
     static const int force_simple = [] { const char* e = getenv("NATS_SOFTMAX_SIMPLE"); return e && atoi(e) != 0; }();
-    if (!force_simple && sample == nullptr && rows <= 148 && V <= kSmCluster * kSmThreads * kSmPer) {
+    if (!force_simple && sample == nullptr && rows <= 132 && V <= kSmCluster * kSmThreads * kSmPer) {
         softmax_cluster_kernel<<<dim3(kSmCluster, rows), kSmThreads, 0, st>>>(logits, V, probs);
         NATS_LAUNCH_OK();
         return 0;

@@ -24,9 +24,9 @@ enum KClass {
     K_OPTIM,
     K_BEAM,
     K_MEMSET,
-    K_TC_GEMM,           // tcgen05 3xTF32, 128 x 128 tiles
-    K_TC_GEMM_SKINNY,    // tcgen05 3xTF32, swapped roles (batch on the N side)
-    K_ENC_PERSIST_FWD,   // persistent weight-stationary tcgen05 bidirectional encoder recurrence (one launch per pass)
+    K_TC_GEMM,           // wgmma 3xTF32, 128 x 64 tiles
+    K_TC_GEMM_SKINNY,    // wgmma 3xTF32, N side <= 64 (the batch, roles swapped)
+    K_ENC_PERSIST_FWD,   // persistent weight-stationary wgmma bidirectional encoder recurrence (one launch per pass)
     K_ENC_PERSIST_BWD,
     K_COUNT
 };

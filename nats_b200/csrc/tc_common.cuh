@@ -1,4 +1,5 @@
-// tc_common.cuh -- device helpers shared by the tcgen05 / TMA kernels (tma_gemm.cu, enc_tc.cu).
+// tc_common.cuh -- device helpers shared by the tensor-core kernels (tc_gemm.cu, enc_tc.cu): mbarriers, TMA box copies and
+// Hopper warpgroup MMAs (wgmma, kind tf32) on K-major SWIZZLE_128B shared-memory operands.
 #pragma once
 #include <cuda.h>
 
@@ -6,10 +7,7 @@
 
 namespace nats {
 
-// host side (tma_gemm.cu): cached 3-D tensor map over a (batch, outer, inner) fp32 array, box = (1, box_outer, 32 floats);
-// mn_major selects the SWIZZLE_128B_ATOM_32B flavour that MN-major tf32 UMMA operands require.
-int tma_map_3d(const float* ptr, long long inner, long long outer, long long ld, long long batch, long long bstride,
-               int box_outer, bool mn_major, CUtensorMap* out);
+// host side (tma_gemm.cu): tensor maps over fp32 arrays
 bool tma_available();
 // plain (unswizzled) 3-D tile map over fp32: dims (d0 contiguous, d1, d2), strides in elements, box (b0, b1, b2)
 int tma_map_tile3d(const float* ptr, long long d0, long long d1, long long d2, long long stride1, long long stride2, int b0,
@@ -26,9 +24,6 @@ __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
 }
 __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx_only(uint64_t* bar, uint32_t bytes) {
-    asm volatile("mbarrier.expect_tx.relaxed.cta.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
 }
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     uint32_t ok;
@@ -49,70 +44,102 @@ __device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* map
         ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
         : "memory");
 }
-// UMMA shared-memory descriptors (cute::UMMA::SmemDescriptor), SWIZZLE_128B
-// non-suspending wait for the single latency-critical threads (MMA issuer): try_wait may park the thread for a
-// scheduler-defined interval when the phase is not complete yet; test_wait returns immediately
-__device__ __forceinline__ void mbar_wait_spin(uint64_t* bar, uint32_t parity) {
-    uint32_t ok;
-    const uint32_t addr = smem_u32(bar);
-    do {
-        asm volatile(
-            "{\n\t.reg .pred p;\n\t"
-            "mbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-            "selp.u32 %0, 1, 0, p;\n\t}"
-            : "=r"(ok)
-            : "r"(addr), "r"(parity)
-            : "memory");
-    } while (!ok);
+// wgmma shared-memory matrix descriptor, K-major SWIZZLE_128B: rows of 128 B (32 tf32), 8-row groups 1024 B apart (stride
+// byte offset), leading byte offset unused; the tile base must be 1024-byte aligned.  Within a 128-byte row the k-step of 8
+// tf32 is selected by advancing the start address by 32 B (+2 in the 16-byte units of the descriptor).
+__device__ __forceinline__ uint64_t desc_sw128(uint32_t saddr) {
+    return (uint64_t)((saddr & 0x3FFFF) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 62);
 }
-__device__ __forceinline__ uint64_t desc_kmajor(uint32_t saddr) {      // rows of 128 B (32 k), 8-row groups 1024 B apart
-    return (uint64_t)((saddr & 0x3FFFF) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) |
-           ((uint64_t)1 << 46) | ((uint64_t)2 << 61);
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across the asynchronous MMAs
+template <int R>
+__device__ __forceinline__ void reg_fence(float (&d)[R]) {
+#pragma unroll
+    for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-// MN-major tf32 operands only exist in the SWIZZLE_128B_BASE32B flavour (cutlass sm100_common.inl:92): rows of 128 B
-// (32 mn) per k, 32-byte chunks XOR (k & 3), K atoms of 4 rows (SBO = 512 B); 32-row mn blocks 4096 B apart (LBO).
-__device__ __forceinline__ uint64_t desc_mnmajor(uint32_t saddr) {
-    return (uint64_t)((saddr & 0x3FFFF) >> 4) | ((uint64_t)(4096 >> 4) << 16) | ((uint64_t)(512 >> 4) << 32) |
-           ((uint64_t)1 << 46) | ((uint64_t)1 << 61);
-}
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc, uint32_t accum) {
+
+// D[64 x N] += A[64 x 8] . B[N x 8]^T, tf32 inputs, fp32 accumulators (d: N/2 registers per thread, fragment i of thread
+// (warp w of the warpgroup, lane l) is row 16w + l/4 + 8*((i/2)&1), column 8*(i/4) + 2*(l&3) + (i&1)).
+// ss: A and B from shared-memory descriptors.  rs: A from registers (a[0..3] = rows l/4, l/4 + 8 x columns l&3, (l&3) + 4).
+__device__ __forceinline__ void wgmma_ss_n32(float (&d)[16], uint64_t da, uint64_t db) {
     asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(da), "l"(db), "r"(idesc), "r"(accum)
-        : "memory");
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(da), "l"(db), "r"(1));
 }
-// A operand read from tensor memory (lane = row m, one 32-bit column per k), B from a shared-memory descriptor
-__device__ __forceinline__ void umma_tf32_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t db, uint32_t idesc, uint32_t accum) {
+__device__ __forceinline__ void wgmma_ss_n64(float (&d)[32], uint64_t da, uint64_t db) {
     asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "r"(tmem_a), "l"(db), "r"(idesc), "r"(accum)
-        : "memory");
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(da), "l"(db), "r"(1));
 }
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t (&r)[16]) {
+__device__ __forceinline__ void wgmma_ss_n128(float (&d)[64], uint64_t da, uint64_t db) {
     asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};"
-        ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-          "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-        : "memory");
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(da), "l"(db), "r"(1));
 }
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
+__device__ __forceinline__ void wgmma_rs_n32(float (&d)[16], const uint32_t (&a)[4], uint64_t db) {
     asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr)
-        : "memory");
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %21, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, {%16,%17,%18,%19}, %20, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(1));
 }
+__device__ __forceinline__ void wgmma_rs_n64(float (&d)[32], const uint32_t (&a)[4], uint64_t db) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, {%32,%33,%34,%35}, %36, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(1));
+}
+
+__device__ __forceinline__ float to_tf32(float x) {
+    uint32_t r;
+    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
+    return __uint_as_float(r);
+}
+__device__ __forceinline__ void st_shared_v4(uint32_t addr, float4 v) {
+    asm volatile("st.shared.v4.f32 [%0], {%1,%2,%3,%4};" ::"r"(addr), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w) : "memory");
+}
+// the tensor core reads the upper 19 bits of an fp32 word: the residual that a raw fp32 operand loses
 __device__ __forceinline__ float resid(float x) { return x - __uint_as_float(__float_as_uint(x) & 0xFFFFE000u); }
 
+// 3xTF32 GEMM epilogue of a warpgroup tile (tc_gemm.cu, tma_gemm.cu): fragment i of this thread is row rb + 8*((i>>1)&1),
+// column cb + 8*(i>>2) + (i&1); value = (acc0 + acc1) + accx (+ bias) (+ old C), stored at C[row*c_rs + col*c_cs]
+template <int R>
+__device__ __forceinline__ void gemm_epilogue(const float (&acc0)[R], const float (&acc1)[R], const float (&accx)[R], float* C,
+                                              long long c_rs, long long c_cs, int Ma, int Nb, int rb, int cb,
+                                              const float* bias_a, const float* bias_n, bool accumulate) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        const int i_row = rb + 8 * h;
+        if (i_row >= Ma) continue;
+        const float ba = bias_a ? __ldg(bias_a + i_row) : 0.f;
+        float* crow = C + (long long)i_row * c_rs;
+#pragma unroll
+        for (int j = 0; j < R / 4; ++j) {
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                const int idx = 4 * j + 2 * h + e;
+                const int col = cb + 8 * j + e;
+                if (col < Nb) {
+                    float o = (acc0[idx] + acc1[idx]) + accx[idx] + ba;
+                    if (bias_n) o += __ldg(bias_n + col);
+                    float* cp = crow + (long long)col * c_cs;
+                    if (accumulate) o += *cp;
+                    *cp = o;
+                }
+            }
+        }
+    }
+}
 
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
     asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");

@@ -1,32 +1,27 @@
-// tc_gemm.cu -- fp32-grade GEMM on the 5th-generation tensor cores: tcgen05.mma kind::tf32 with the 3xTF32 split
+// tc_gemm.cu -- fp32-grade GEMM on the Hopper tensor cores: wgmma kind::tf32 with the 3xTF32 split
 //   x = hi + lo,  hi = rna_tf32(x),  lo = rna_tf32(x - hi);   a.b ~= a_hi.b_hi + a_hi.b_lo + a_lo.b_hi
-// (error ~1e-6 relative per product, i.e. fp32 grade -- the parity tests keep their fp32 tolerances).
-// The tensor core truncates the fp32 accumulator once per MMA (measured: error grows linearly with the chain
-// length), so the accumulation is spread over FOUR TMEM accumulators: the hi.hi products go round-robin into three
-// "main" accumulators (chain length K/24 instead of 3K/8) and the two small cross terms into a fourth; the epilogue
-// adds the four with ordinary round-to-nearest fp32 adds.
+// (error ~1e-6 relative per product, i.e. fp32 grade -- the parity tests keep their fp32 tolerances).  The hi.hi products
+// alternate between two register accumulators and the two small cross terms go to a third, so that each accumulation
+// chain is short; the epilogue adds the three with ordinary round-to-nearest fp32 adds.
 //
-// One CTA computes a [128 x BN] accumulator tile that lives in TENSOR MEMORY (BN columns x 128 lanes, fp32):
-//   warps 0-7  (256 thr) loaders : global -> registers -> {hi,lo} split -> st.shared into the canonical K-major
-//                                  SWIZZLE_128B operand layout (row = 128 B = 32 tf32, 16-byte chunk c of row r
-//                                  stored at chunk c ^ (r & 7)); handles K-contiguous AND row-contiguous sources,
-//                                  so every transposition of the caller maps to the same K-major descriptors
-//   warp  8    (1 lane)  issuer  : waits on the stage's mbarrier, issues 4 k-steps x 3 tcgen05.mma (UMMA 128xBNx8),
-//                                  tcgen05.commit -> frees the stage / signals the epilogue
-//   warps 8-11 (128 thr) epilogue: tcgen05.ld 32x32b.x32 (TMEM -> registers), bias / accumulate / split-K slab, store
-// Pipelines: smem ring full[]/empty[] mbarriers (loaders <-> tensor core), one accumulator barrier (MMA -> epilogue).
+// One CTA (two warpgroups, 256 threads) computes a [128 x BN] tile, warpgroup w owning rows 64w..64w+63:
+//   every thread loads its share of the next 32-deep k-block from global memory into registers while the tensor cores
+//   work on the current one, splits it into {hi, lo} and stores both into the other shared-memory stage in the canonical
+//   K-major SWIZZLE_128B layout (row = 128 B = 32 tf32, 16-byte chunk c of row r stored at chunk c ^ (r & 7)).  The loader
+//   handles K-contiguous AND row-contiguous sources, so every transposition of the caller maps to the same K-major
+//   operands (tf32 wgmma reads K-major shared-memory operands only).
+//   per k-block and warpgroup: 4 k-steps x 3 wgmma m64 x BN x 8, then a wait before that stage is written again.
 // Operand roles are chosen by the host so that the 128-row side is the larger one (skinny recurrent products run
 // "swapped": the weight matrix is the 128-row operand, the batch is the N side, the store is transposed).
 #include "gemm.cuh"
+#include "tc_common.cuh"
 
 namespace nats {
 
 namespace {
 
-constexpr int kTcLoaderThreads = 256;
-constexpr int kTcThreads = 384;
+constexpr int kTcThreads = 256;
 constexpr int kTcBlockK = 32;        // tf32 elements per k-block = one 128-byte swizzle row
-constexpr int kTcUmmaK = 8;          // tf32 MMA K
 constexpr int kTcMaxGroup = 4;
 
 struct TcProblem {
@@ -49,78 +44,20 @@ struct TcGroup {
     int count;
 };
 
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-    uint32_t ok;
-    const uint32_t addr = smem_u32(bar);
-    do {
-        asm volatile(
-            "{\n\t.reg .pred p;\n\t"
-            "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-            "selp.u32 %0, 1, 0, p;\n\t}"
-            : "=r"(ok)
-            : "r"(addr), "r"(parity)
-            : "memory");
-    } while (!ok);
-}
-__device__ __forceinline__ float to_tf32(float x) {
-    uint32_t r;
-    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
-    return __uint_as_float(r);
-}
-__device__ __forceinline__ float trunc_tf32(float x) { return __uint_as_float(__float_as_uint(x) & 0xFFFFE000u); }
-__device__ __forceinline__ void st_shared_v4(uint32_t addr, float4 v) {
-    asm volatile("st.shared.v4.f32 [%0], {%1,%2,%3,%4};" ::"r"(addr), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w) : "memory");
-}
-// K-major, SWIZZLE_128B shared-memory matrix descriptor (cute::UMMA::SmemDescriptor): 8-row groups 1024 B apart
-__device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr) {
-    uint64_t d = 0;
-    d |= (uint64_t)((saddr & 0x3FFFF) >> 4);          // start address, 16-byte units, bits [0,14)
-    d |= (uint64_t)1 << 16;                           // leading byte offset (unused for swizzled K-major), [16,30)
-    d |= (uint64_t)(1024 >> 4) << 32;                 // stride byte offset between 8-row groups, [32,46)
-    d |= (uint64_t)1 << 46;                           // descriptor version (Blackwell), [46,48)
-    d |= (uint64_t)2 << 61;                           // layout type SWIZZLE_128B, [61,64)
-    return d;
-}
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc, uint32_t accum) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(da), "l"(db), "r"(idesc), "r"(accum)
-        : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr)
-        : "memory");
-}
+using namespace tc;
 
 // one operand tile: ROWS x 32 tf32, read from global with arbitrary (row, k) strides, written as hi/lo K-major tiles
 template <int ROWS>
 struct TileLoader {
     static constexpr int kChunks = ROWS * 8;                                  // 16-byte chunks (4 k each)
-    static constexpr int kPer = (kChunks + kTcLoaderThreads - 1) / kTcLoaderThreads;
+    static constexpr int kPer = (kChunks + kTcThreads - 1) / kTcThreads;
     float4 v[kPer];
 
     __device__ __forceinline__ void load(const float* __restrict__ g, long long rs, long long ks, int row0, int nrows,
                                          int k0, int kend, bool vec_ok, int tid) {
 #pragma unroll
         for (int i = 0; i < kPer; ++i) {
-            const int q = tid + i * kTcLoaderThreads;
+            const int q = tid + i * kTcThreads;
             float4 val = make_float4(0.f, 0.f, 0.f, 0.f);
             if (q < kChunks) {
                 int r, c;
@@ -145,23 +82,16 @@ struct TileLoader {
     __device__ __forceinline__ void store(uint32_t hi_base, uint32_t lo_base, long long ks, int tid) const {
 #pragma unroll
         for (int i = 0; i < kPer; ++i) {
-            const int q = tid + i * kTcLoaderThreads;
+            const int q = tid + i * kTcThreads;
             if (q < kChunks) {
                 int r, c;
                 if (ks == 1) { r = q >> 3; c = q & 7; }
                 else { r = q % ROWS; c = q / ROWS; }
                 const uint32_t off = (uint32_t)(r * 128 + ((c ^ (r & 7)) << 4));
                 float4 hi, lo;
-#ifdef NATS_TC_RAW_HI
-                // experiment: feed the raw fp32 word as "hi" (the tensor core is assumed to truncate to tf32)
-                hi = v[i];
-                lo.x = v[i].x - trunc_tf32(v[i].x); lo.y = v[i].y - trunc_tf32(v[i].y);
-                lo.z = v[i].z - trunc_tf32(v[i].z); lo.w = v[i].w - trunc_tf32(v[i].w);
-#else
                 hi.x = to_tf32(v[i].x); hi.y = to_tf32(v[i].y); hi.z = to_tf32(v[i].z); hi.w = to_tf32(v[i].w);
                 lo.x = to_tf32(v[i].x - hi.x); lo.y = to_tf32(v[i].y - hi.y);
                 lo.z = to_tf32(v[i].z - hi.z); lo.w = to_tf32(v[i].w - hi.w);
-#endif
                 st_shared_v4(hi_base + off, hi);
                 st_shared_v4(lo_base + off, lo);
             }
@@ -169,19 +99,21 @@ struct TileLoader {
     }
 };
 
-template <int BN, int STAGES>
+template <int BN>
+__device__ __forceinline__ void mma_bn(float (&d)[BN / 2], uint64_t da, uint64_t db) {
+    if constexpr (BN == 32) wgmma_ss_n32(d, da, db);
+    else wgmma_ss_n64(d, da, db);
+}
+
+template <int BN>
 __global__ void __launch_bounds__(kTcThreads, 1) tc_gemm_kernel(const __grid_constant__ TcGroup grp) {
     constexpr uint32_t kABytes = 128 * 128;                 // one 128-row operand tile (hi or lo)
     constexpr uint32_t kBBytes = BN * 128;
     constexpr uint32_t kStageBytes = 2 * kABytes + 2 * kBBytes;
-    constexpr uint32_t kTmemCols = 4 * BN;                  // main0 | main1 | main2 | corr ; power of two >= 32
-    static_assert(BN == 32 || BN == 64 || BN == 128, "BN");
+    constexpr int R = BN / 2;                               // accumulator registers per thread
+    static_assert(BN == 32 || BN == 64, "BN");
 
     extern __shared__ __align__(1024) unsigned char smem[];
-    __shared__ __align__(8) uint64_t full_bar[STAGES];
-    __shared__ __align__(8) uint64_t empty_bar[STAGES];
-    __shared__ __align__(8) uint64_t accum_bar;
-    __shared__ uint32_t tmem_base_slot;
 
     int z = blockIdx.z, g = 0;
 #pragma unroll
@@ -197,160 +129,72 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_gemm_kernel(const __grid_con
     const int kend = min(P.K, kbeg + P.kchunk);
     const int nkb = (kend > kbeg) ? (kend - kbeg + kTcBlockK - 1) / kTcBlockK : 0;
 
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = tid >> 7;
     const uint32_t smem_base = (smem_u32(smem) + 1023u) & ~1023u;   // SWIZZLE_128B tiles need 1024-byte alignment
-
-    if (tid == 0) {
-        for (int s = 0; s < STAGES; ++s) {
-            mbar_init(&full_bar[s], kTcLoaderThreads);
-            mbar_init(&empty_bar[s], 1);
-        }
-        mbar_init(&accum_bar, 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 8) {                                        // TMEM allocation is warp-wide (.sync.aligned)
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_base_slot)),
-                     "r"(kTmemCols)
-                     : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_d = tmem_base_slot;
     pdl_trigger();
     pdl_wait();
 
-    if (warp < 8) {
-        // ===================== loaders =====================
-        const float* __restrict__ A = P.A + (long long)batch * P.sA;
-        const float* __restrict__ B = P.B + (long long)batch * P.sB;
-        const bool vecA = (P.a_ks == 1) && ((P.a_rs & 3) == 0) && ((reinterpret_cast<uintptr_t>(A) & 15) == 0);
-        const bool vecB = (P.b_ks == 1) && ((P.b_rs & 3) == 0) && ((reinterpret_cast<uintptr_t>(B) & 15) == 0);
-        TileLoader<128> la;
-        TileLoader<BN> lb;
-        if (nkb > 0) {
-            la.load(A, P.a_rs, P.a_ks, m0, P.Ma, kbeg, kend, vecA, tid);
-            lb.load(B, P.b_rs, P.b_ks, n0, P.Nb, kbeg, kend, vecB, tid);
-        }
-        for (int kb = 0; kb < nkb; ++kb) {
-            const int s = kb % STAGES;
-            const uint32_t par = (uint32_t)((kb / STAGES) & 1);
-            mbar_wait(&empty_bar[s], par ^ 1u);             // stage drained by the tensor core
-            const uint32_t st = smem_base + (uint32_t)s * kStageBytes;
-            la.store(st, st + kABytes, P.a_ks, tid);
-            lb.store(st + 2 * kABytes, st + 2 * kABytes + kBBytes, P.b_ks, tid);
-            if (kb + 1 < nkb) {                             // next tile's global loads fly while this one is consumed
-                const int k0 = kbeg + (kb + 1) * kTcBlockK;
-                la.load(A, P.a_rs, P.a_ks, m0, P.Ma, k0, kend, vecA, tid);
-                lb.load(B, P.b_rs, P.b_ks, n0, P.Nb, k0, kend, vecB, tid);
-            }
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> async proxy (UMMA)
-            mbar_arrive(&full_bar[s]);
-        }
-    } else {
-        // ===================== MMA issuer (one lane of warp 8) =====================
-        if (warp == 8 && lane == 0) {
-            const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(BN >> 3) << 17) | ((128u >> 4) << 24);
-            for (int kb = 0; kb < nkb; ++kb) {
-                const int s = kb % STAGES;
-                mbar_wait(&full_bar[s], (uint32_t)((kb / STAGES) & 1));
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                const uint32_t st = smem_base + (uint32_t)s * kStageBytes;
-                const uint64_t a_hi = make_smem_desc(st), a_lo = make_smem_desc(st + kABytes);
-                const uint64_t b_hi = make_smem_desc(st + 2 * kABytes), b_lo = make_smem_desc(st + 2 * kABytes + kBBytes);
+    float acc0[R], acc1[R], accx[R];
 #pragma unroll
-                for (int kk = 0; kk < kTcBlockK / kTcUmmaK; ++kk) {
-                    const uint64_t adv = (uint64_t)((kk * kTcUmmaK * 4) >> 4);   // +32 bytes per k-step inside the swizzle row
-                    const int gstep = kb * (kTcBlockK / kTcUmmaK) + kk;
-                    umma_tf32(tmem_d + 3u * BN, a_lo + adv, b_hi + adv, idesc, gstep != 0 ? 1u : 0u);
-                    umma_tf32(tmem_d + 3u * BN, a_hi + adv, b_lo + adv, idesc, 1u);
-                    umma_tf32(tmem_d + (uint32_t)(gstep % 3) * BN, a_hi + adv, b_hi + adv, idesc, gstep >= 3 ? 1u : 0u);
-                }
-                umma_commit(&empty_bar[s]);                 // arrives when the MMAs above have read the stage
-            }
-            umma_commit(&accum_bar);                        // accumulator complete
-        }
-        __syncwarp();
-        // ===================== epilogue (warps 8-11 <-> TMEM lanes 0-127) =====================
-        const int q = warp - 8;
-        const int i = m0 + q * 32 + lane;                   // A-side row owned by this thread
-        float* __restrict__ C = P.C + (long long)batch * P.sC + (long long)split * P.strideP;
-        const bool add_bias = (P.bias != nullptr) && (split == 0);
-        if (nkb > 0) {
-            mbar_wait(&accum_bar, 0);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        }
-        const float bias_a = (add_bias && P.bias_on_a && i < P.Ma) ? __ldg(P.bias + i) : 0.f;
-#pragma unroll 1
-        for (int c0 = 0; c0 < BN; c0 += 16) {
-            if (n0 + c0 >= P.Nb) break;                     // warp-uniform
-            float r[16];
-            if (nkb > 0) {
-                uint32_t t0[16], t1[16], t2[16], t3[16];
-                const uint32_t ta = tmem_d + ((uint32_t)(q * 32) << 16) + (uint32_t)c0;
-                tmem_ld16(ta, t0);
-                tmem_ld16(ta + BN, t1);
-                tmem_ld16(ta + 2 * BN, t2);
-                tmem_ld16(ta + 3 * BN, t3);
-                asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-                for (int t = 0; t < 16; ++t)
-                    r[t] = ((__uint_as_float(t0[t]) + __uint_as_float(t1[t])) + __uint_as_float(t2[t])) + __uint_as_float(t3[t]);
-            } else {
-#pragma unroll
-                for (int t = 0; t < 16; ++t) r[t] = 0.f;
-            }
-            if (i < P.Ma) {
-                float* crow = C + (long long)i * P.c_rs;
-                const bool vec = (P.c_cs == 1) && ((P.c_rs & 3) == 0) && ((reinterpret_cast<uintptr_t>(C) & 15) == 0) &&
-                                 (n0 + c0 + 15 < P.Nb);
-                if (vec) {
-#pragma unroll
-                    for (int t = 0; t < 16; t += 4) {
-                        const int j = n0 + c0 + t;
-                        float4 o = make_float4(r[t] + bias_a, r[t + 1] + bias_a, r[t + 2] + bias_a, r[t + 3] + bias_a);
-                        if (add_bias && !P.bias_on_a) {
-                            o.x += __ldg(P.bias + j); o.y += __ldg(P.bias + j + 1);
-                            o.z += __ldg(P.bias + j + 2); o.w += __ldg(P.bias + j + 3);
-                        }
-                        float4* cp = reinterpret_cast<float4*>(crow + j);
-                        if (P.accumulate) {
-                            const float4 old = *cp;
-                            o.x += old.x; o.y += old.y; o.z += old.z; o.w += old.w;
-                        }
-                        *cp = o;
-                    }
-                } else {
-#pragma unroll
-                    for (int t = 0; t < 16; ++t) {
-                        const int j = n0 + c0 + t;
-                        if (j < P.Nb) {
-                            float o = r[t] + bias_a;
-                            if (add_bias && !P.bias_on_a) o += __ldg(P.bias + j);
-                            float* cp = crow + (long long)j * P.c_cs;
-                            if (P.accumulate) o += *cp;
-                            *cp = o;
-                        }
-                    }
-                }
-            }
-        }
+    for (int i = 0; i < R; ++i) { acc0[i] = 0.f; acc1[i] = 0.f; accx[i] = 0.f; }
+
+    const float* __restrict__ A = P.A + (long long)batch * P.sA;
+    const float* __restrict__ B = P.B + (long long)batch * P.sB;
+    const bool vecA = (P.a_ks == 1) && ((P.a_rs & 3) == 0) && ((reinterpret_cast<uintptr_t>(A) & 15) == 0);
+    const bool vecB = (P.b_ks == 1) && ((P.b_rs & 3) == 0) && ((reinterpret_cast<uintptr_t>(B) & 15) == 0);
+    TileLoader<128> la;
+    TileLoader<BN> lb;
+    if (nkb > 0) {
+        la.load(A, P.a_rs, P.a_ks, m0, P.Ma, kbeg, kend, vecA, tid);
+        lb.load(B, P.b_rs, P.b_ks, n0, P.Nb, kbeg, kend, vecB, tid);
+        la.store(smem_base, smem_base + kABytes, P.a_ks, tid);
+        lb.store(smem_base + 2 * kABytes, smem_base + 2 * kABytes + kBBytes, P.b_ks, tid);
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> async proxy (wgmma)
     __syncthreads();
-    if (warp == 8) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_d), "r"(kTmemCols) : "memory");
+    for (int kb = 0; kb < nkb; ++kb) {
+        const uint32_t st = smem_base + (uint32_t)(kb & 1) * kStageBytes;
+        const bool next = kb + 1 < nkb;
+        if (next) {                                         // next tile's global loads fly while this one is consumed
+            const int k0 = kbeg + (kb + 1) * kTcBlockK;
+            la.load(A, P.a_rs, P.a_ks, m0, P.Ma, k0, kend, vecA, tid);
+            lb.load(B, P.b_rs, P.b_ks, n0, P.Nb, k0, kend, vecB, tid);
+        }
+        const uint64_t a_hi = desc_sw128(st + (uint32_t)wg * (kABytes / 2)), a_lo = desc_sw128(st + kABytes + (uint32_t)wg * (kABytes / 2));
+        const uint64_t b_hi = desc_sw128(st + 2 * kABytes), b_lo = desc_sw128(st + 2 * kABytes + kBBytes);
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < kTcBlockK / 8; ++kk) {
+            const uint64_t adv = (uint64_t)(kk * 2);          // +32 bytes per k-step inside the swizzle row
+            mma_bn<BN>(accx, a_lo + adv, b_hi + adv);
+            mma_bn<BN>(accx, a_hi + adv, b_lo + adv);
+            mma_bn<BN>((kk & 1) ? acc1 : acc0, a_hi + adv, b_hi + adv);
+        }
+        wgmma_commit();
+        if (next) {                                         // the other stage was drained by the wait of the previous k-block
+            const uint32_t nx = smem_base + (uint32_t)((kb + 1) & 1) * kStageBytes;
+            la.store(nx, nx + kABytes, P.a_ks, tid);
+            lb.store(nx + 2 * kABytes, nx + 2 * kABytes + kBBytes, P.b_ks, tid);
+        }
+        wgmma_wait<0>();
+        reg_fence(acc0); reg_fence(acc1); reg_fence(accx);
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+        __syncthreads();
     }
+
+    const bool add_bias = (P.bias != nullptr) && (split == 0);
+    gemm_epilogue(acc0, acc1, accx, P.C + (long long)batch * P.sC + (long long)split * P.strideP, P.c_rs, P.c_cs, P.Ma, P.Nb,
+                  m0 + 64 * wg + 16 * (warp & 3) + (lane >> 2), n0 + 2 * (lane & 3), (add_bias && P.bias_on_a) ? P.bias : nullptr,
+                  (add_bias && !P.bias_on_a) ? P.bias : nullptr, P.accumulate != 0);
 }
 
-template <int BN, int STAGES>
+template <int BN>
 constexpr size_t tc_smem_bytes() {
-    return (size_t)STAGES * (2 * 128 * 128 + 2 * BN * 128) + 1024;
+    return (size_t)2 * (2 * 128 * 128 + 2 * BN * 128) + 1024;
 }
 
-template <int BN, int STAGES>
-int tc_launch(cudaStream_t st, const TcGroup& grp) {
+template <int BN>
+int tc_launch(cudaStream_t st, const TcGroup& grp, bool skinny) {
     int ga = 0, gb = 0;
     double flops = 0.0, bytes = 0.0;
     for (int i = 0; i < grp.count; ++i) {
@@ -362,15 +206,9 @@ int tc_launch(cudaStream_t st, const TcGroup& grp) {
     }
     const int gz = grp.zstart[grp.count];
     if (ga == 0 || gb == 0 || gz == 0) return 0;
-    static bool attr_set = false;
-    if (!attr_set) {
-        NATS_CUDA_OK(cudaFuncSetAttribute(tc_gemm_kernel<BN, STAGES>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                          (int)tc_smem_bytes<BN, STAGES>()));
-        attr_set = true;
-    }
-    ProfScope ps(st, BN <= 64 ? K_TC_GEMM_SKINNY : K_TC_GEMM, flops, bytes);
+    ProfScope ps(st, skinny ? K_TC_GEMM_SKINNY : K_TC_GEMM, flops, bytes);
     dim3 grid(ga, gb, gz);
-    NATS_CUDA_OK(launch_pdl(tc_gemm_kernel<BN, STAGES>, grid, dim3(kTcThreads), tc_smem_bytes<BN, STAGES>(), st, grp));
+    NATS_CUDA_OK(launch_pdl(tc_gemm_kernel<BN>, grid, dim3(kTcThreads), tc_smem_bytes<BN>(), st, grp));
     return 0;
 }
 
@@ -378,12 +216,8 @@ int tc_launch(cudaStream_t st, const TcGroup& grp) {
 
 // One-time kernel attribute setup (must not happen lazily inside a stream capture).
 int tc_gemm_setup() {
-    NATS_CUDA_OK(cudaFuncSetAttribute(tc_gemm_kernel<32, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                      (int)tc_smem_bytes<32, 4>()));
-    NATS_CUDA_OK(cudaFuncSetAttribute(tc_gemm_kernel<64, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                      (int)tc_smem_bytes<64, 4>()));
-    NATS_CUDA_OK(cudaFuncSetAttribute(tc_gemm_kernel<128, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                      (int)tc_smem_bytes<128, 3>()));
+    NATS_CUDA_OK(cudaFuncSetAttribute(tc_gemm_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc_smem_bytes<32>()));
+    NATS_CUDA_OK(cudaFuncSetAttribute(tc_gemm_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc_smem_bytes<64>()));
     return 0;
 }
 
@@ -400,7 +234,7 @@ int tc_gemm_launch(cudaStream_t st, const GemmProblem* probs, int count, bool tr
     // operand roles: the 128-row side should be the larger dimension
     const bool swapped = maxM < 128 && maxN > maxM;
     const int nb_dim = swapped ? maxM : maxN;
-    const int BN = nb_dim <= 32 ? 32 : (nb_dim <= 64 ? 64 : 128);
+    const int BN = nb_dim <= 32 ? 32 : 64;
     for (int i = 0; i < count; ++i) {
         const GemmProblem& q = probs[i];
         NATS_REQUIRE(q.splitk >= 1 && q.batch >= 1 && (q.splitk == 1 || !q.accumulate), "tc gemm split/batch");
@@ -431,9 +265,7 @@ int tc_gemm_launch(cudaStream_t st, const GemmProblem* probs, int count, bool tr
     }
     grp.zstart[count] = z;
     for (int i = count; i < kTcMaxGroup; ++i) grp.zstart[i + 1] = z;
-    if (BN == 32) return tc_launch<32, 4>(st, grp);
-    if (BN == 64) return tc_launch<64, 4>(st, grp);
-    return tc_launch<128, 3>(st, grp);
+    return BN == 32 ? tc_launch<32>(st, grp, true) : tc_launch<64>(st, grp, nb_dim <= 64);
 }
 
 }  // namespace nats

@@ -1,693 +1,27 @@
-// tma_gemm.cu -- tcgen05 3xTF32 GEMM fed by the Tensor Memory Accelerator.
+// tma_gemm.cu -- 3xTF32 GEMM on wgmma fed by the Tensor Memory Accelerator, and the host side of TMA (tensor maps).
 //
-//   TMA (cp.async.bulk.tensor.2d/3d, SWIZZLE_128B) lands RAW fp32 operand tiles straight in the canonical UMMA
-//   shared-memory layout -- K-major for K-contiguous sources, MN-major for row-contiguous sources, so no transposed
-//   copies of anything are ever made.  The tensor core truncates fp32 words to tf32 (verified on B200), hence the raw
-//   tile IS the "hi" operand; eight warps only compute the residual tiles  lo = x - trunc_tf32(x)  in shared memory.
-//       D += A_lo.B_raw + A_raw.B_lo          (correction accumulator)
-//       D += A_raw.B_raw                      (three round-robin main accumulators: short truncation chains)
-//   warp 8 lane 0 : TMA producer        (waits empty[s], arms tma_full[s] with expect_tx, issues the box copies)
-//   warps 0-7     : residual pass        (wait tma_full[s]; raw -> lo, 16-byte vectors; fence.proxy.async; arrive mma_full[s])
-//   warp 9 lane 0 : tcgen05.mma issuer   (wait mma_full[s]; 4 k-steps x 3 UMMA 128 x BN x 8; tcgen05.commit -> empty[s])
-//   warps 8-11    : epilogue             (tcgen05.ld of the four accumulators, fp32 sum, bias/accumulate/slab store)
-// Two kernels share the host side (tensor-map cache, grouping, split-K, PDL launch):
-//   tma_gemm_kernel     both operands from shared memory (above); used for the 128-wide tiles;
-//   tma_gemm_ts_kernel  skinny products (the batch, <= 64, on the N side): the 128-row weight operand goes through
-//                       TENSOR MEMORY (split warps tcgen05.st hi and lo; TS-form MMA) and the two products sharing A_hi
-//                       are stacked along N -- 2 MMAs per k-step, 56 KB instead of 120 KB of shared-memory traffic per
-//                       16 KB weight tile.  Default for BN <= 64 (NATS_TS=0: off).
+//   Thread 0 keeps a ring of NR raw stages filled with cp.async.bulk.tensor boxes of 32 k x rows of both operands,
+//   straight from the caller's layout (K-contiguous or row-contiguous sources: no transposed copies are ever made).
+//   The 256 threads (two warpgroups, rows 64w..64w+63 of the 128-row tile) split the next raw stage into tf32 {hi, lo}
+//   K-major SWIZZLE_128B tiles (the only layout tf32 wgmma reads) while the tensor cores work on the current one:
+//       D += A_hi.B_hi (two alternating accumulators),   D += A_lo.B_hi + A_hi.B_lo (a third).
+//   Skinny products (the batch, <= 64, on the N side; NATS_TS=1, the default): the 128-row operand (the weights) is NOT
+//   split into shared memory -- each thread reads its wgmma A fragments straight from the raw stage, splits them in
+//   registers and issues the register-A form, so only the small B operand goes through the split pass.
 // Requirements: 16-byte aligned base pointers and leading dimensions that are multiples of 4 floats (TMA strides);
 // anything else is served by the software-loader kernel in tc_gemm.cu.
 #include <cuda.h>
 
 #include <unordered_map>
-#include <string>
 
 #include "gemm.cuh"
+#include "ops.cuh"
 #include "tc_common.cuh"
 
 namespace nats {
 
 namespace {
 
-constexpr int kThreads = 384;
-constexpr int kSplitThreads = 256;
-constexpr int kBlockK = 32;
-constexpr int kMaxGroup = 2;
-
-struct TmaProblem {
-    float* C;
-    const float* bias;
-    int Ma, Nb, K;
-    long long c_rs, c_cs;
-    int batch;
-    long long sC;
-    int splitk, kchunk;
-    long long strideP;
-    int accumulate;
-    int bias_on_a;
-    int a_static;        // the 128-row operand is constant within the step (weights): may be prefetched before pdl_wait
-};
-struct alignas(64) TmaGroup {
-    CUtensorMap mapA[kMaxGroup];
-    CUtensorMap mapB[kMaxGroup];
-    TmaProblem p[kMaxGroup];
-    int zstart[kMaxGroup + 1];
-    int count;
-    int trace;           // debug: CTA (0,0,0) prints its phase timestamps (NATS_TRACE)
-    int dbg_mode;        // debug timing experiments (WRONG results): 1 = skip the residual arithmetic, 2 = hi*hi product only
-};
-
-using namespace tc;
-
-template <int BN, int NR, int NL, bool A_MN, bool B_MN>
-__global__ void __launch_bounds__(kThreads, 1) tma_gemm_kernel(const __grid_constant__ TmaGroup grp) {
-    // shared memory: NR raw stages [A_raw 16 KB | B_raw BN*128] (filled by TMA, deep: covers the TMA latency) and
-    //                NL residual stages [A_lo | B_lo] (written by the residual warps, shallow: only lives until its MMAs retire)
-    constexpr uint32_t kABytes = 128 * 128, kBBytes = BN * 128;
-    constexpr uint32_t kRawStage = kABytes + kBBytes;
-    constexpr uint32_t kLoBase = NR * kRawStage;
-    constexpr uint32_t kTmemCols = 4 * BN;
-
-    extern __shared__ __align__(1024) unsigned char smem[];
-    __shared__ __align__(8) uint64_t tma_full[NR];
-    __shared__ __align__(8) uint64_t raw_empty[NR];
-    __shared__ __align__(8) uint64_t lo_full[NL];
-    __shared__ __align__(8) uint64_t lo_empty[NL];
-    __shared__ __align__(8) uint64_t accum_bar;
-    __shared__ uint32_t tmem_base_slot;
-    __shared__ unsigned long long tr_s[16];
-#ifdef NATS_TRACE_BUILD
-    const bool tr = grp.trace && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0;
-#else
-    constexpr bool tr = false;
-#endif
-    if (tr && threadIdx.x == 0) tr_s[0] = gtimer();
-
-    int z = blockIdx.z, g = 0;
-    if (grp.count > 1 && z >= grp.zstart[1]) g = 1;
-    const TmaProblem& P = grp.p[g];
-    const CUtensorMap* mapA = &grp.mapA[g];
-    const CUtensorMap* mapB = &grp.mapB[g];
-    z -= grp.zstart[g];
-    const int split = z % P.splitk, batch = z / P.splitk;
-    const int m0 = blockIdx.x * 128, n0 = blockIdx.y * BN;
-    if (m0 >= P.Ma || n0 >= P.Nb) return;
-
-    const int kbeg = split * P.kchunk;
-    const int kend = min(P.K, kbeg + P.kchunk);
-    const int nkb = (kend > kbeg) ? (kend - kbeg + kBlockK - 1) / kBlockK : 0;
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const uint32_t smem_base = (smem_u32(smem) + 1023u) & ~1023u;
-
-    if (tid == 0) {
-        // descriptor fetch off the critical path (the B tiles are requested right after the dependency wait)
-        asm volatile("prefetch.tensormap [%0];" ::"l"(mapA) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(mapB) : "memory");
-        for (int s = 0; s < NR; ++s) { mbar_init(&tma_full[s], 1); mbar_init(&raw_empty[s], 1); }
-        for (int s = 0; s < NL; ++s) { mbar_init(&lo_full[s], kSplitThreads / 32); mbar_init(&lo_empty[s], 1); }
-        mbar_init(&accum_bar, 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 8) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_base_slot)),
-                     "r"(kTmemCols)
-                     : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_d = tmem_base_slot;
-    if (tr && tid == 0) tr_s[1] = gtimer();
-    pdl_trigger();                      // dependents may launch now (they block in their own pdl_wait)
-
-    if (warp < 8) {
-        // ===================== residual pass: lo = raw - trunc_tf32(raw) =====================
-        for (int kb = 0; kb < nkb; ++kb) {
-            const int sr = kb % NR, sl = kb % NL;
-            mbar_wait(&lo_empty[sl], (uint32_t)(((kb / NL) & 1) ^ 1));      // residual slot drained by the tensor core
-            mbar_wait(&tma_full[sr], (uint32_t)((kb / NR) & 1));            // raw tiles landed
-            if (tr && tid == 0 && kb == 0) tr_s[5] = gtimer();
-            const uint32_t raw = smem_base + (uint32_t)sr * kRawStage;
-            const uint32_t lo = smem_base + kLoBase + (uint32_t)sl * kRawStage;
-            if (grp.dbg_mode != 1)
-#pragma unroll
-            for (int i = 0; i < (int)(kRawStage / 16 + kSplitThreads - 1) / kSplitThreads; ++i) {
-                const uint32_t q = (uint32_t)(tid + i * kSplitThreads);
-                if (q < kRawStage / 16) {
-                    float4 v;
-                    asm volatile("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(raw + q * 16u));
-                    asm volatile("st.shared.v4.f32 [%0], {%1,%2,%3,%4};" ::"r"(lo + q * 16u), "f"(resid(v.x)), "f"(resid(v.y)),
-                                 "f"(resid(v.z)), "f"(resid(v.w))
-                                 : "memory");
-                }
-            }
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&lo_full[sl]);                        // one arrival per warp
-        }
-        if (tr && tid == 0) tr_s[6] = gtimer();
-    } else {
-        if (warp == 8 && lane == 0) {
-            // ===================== TMA producer =====================
-            // With PDL the predecessor kernel may still be running: operands it produces must not be read before
-            // pdl_wait().  When `a_static` (the 128-row operand is a weight matrix, constant within the step) its
-            // tiles for the first ring fill are prefetched BEFORE the wait.
-            const int npre = P.a_static ? min(nkb, NR) : 0;
-            for (int kb = 0; kb < npre; ++kb) {
-                const uint32_t raw = smem_base + (uint32_t)kb * kRawStage;
-                const int k0 = kbeg + kb * kBlockK;
-                mbar_expect_tx_only(&tma_full[kb], kABytes);
-                if (A_MN) {
-#pragma unroll
-                    for (int bi = 0; bi < 4; ++bi) tma_load_3d(raw + bi * 4096, mapA, &tma_full[kb], m0 + 32 * bi, k0, batch);
-                } else {
-                    tma_load_3d(raw, mapA, &tma_full[kb], k0, m0, batch);
-                }
-            }
-            if (tr) tr_s[2] = gtimer();
-            pdl_wait();
-            if (tr) tr_s[3] = gtimer();
-            for (int kb = 0; kb < nkb; ++kb) {
-                const int sr = kb % NR;
-                mbar_wait(&raw_empty[sr], (uint32_t)(((kb / NR) & 1) ^ 1));
-                const uint32_t raw = smem_base + (uint32_t)sr * kRawStage;
-                const int k0 = kbeg + kb * kBlockK;
-                if (kb < npre) {                  // A already in flight: only B left for this stage
-                    mbar_expect_tx(&tma_full[sr], kBBytes);
-                    if (B_MN) {
-#pragma unroll
-                        for (int bi = 0; bi < BN / 32; ++bi)
-                            tma_load_3d(raw + kABytes + bi * 4096, mapB, &tma_full[sr], n0 + 32 * bi, k0, batch);
-                    } else {
-                        tma_load_3d(raw + kABytes, mapB, &tma_full[sr], k0, n0, batch);
-                    }
-                    continue;
-                }
-                mbar_expect_tx(&tma_full[sr], kRawStage);
-                if (A_MN) {
-#pragma unroll
-                    for (int bi = 0; bi < 4; ++bi) tma_load_3d(raw + bi * 4096, mapA, &tma_full[sr], m0 + 32 * bi, k0, batch);
-                } else {
-                    tma_load_3d(raw, mapA, &tma_full[sr], k0, m0, batch);
-                }
-                if (B_MN) {
-#pragma unroll
-                    for (int bi = 0; bi < BN / 32; ++bi)
-                        tma_load_3d(raw + kABytes + bi * 4096, mapB, &tma_full[sr], n0 + 32 * bi, k0, batch);
-                } else {
-                    tma_load_3d(raw + kABytes, mapB, &tma_full[sr], k0, n0, batch);
-                }
-            }
-            if (tr) tr_s[4] = gtimer();
-        } else if (warp == 9 && lane == 0) {
-            // ===================== MMA issuer =====================
-            const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((A_MN ? 1u : 0u) << 15) | ((B_MN ? 1u : 0u) << 16) |
-                                   ((uint32_t)(BN >> 3) << 17) | ((128u >> 4) << 24);
-            // straight-line issue code (see enc_tc.cu / the TS kernel below): first k-block peeled, accumulator of a k-step
-            // fixed by its position in the block, ring indices as running counters, descriptors advanced by constants
-            const uint64_t a_raw0 = A_MN ? desc_mnmajor(smem_base) : desc_kmajor(smem_base);
-            const uint64_t b_raw0 = B_MN ? desc_mnmajor(smem_base + kABytes) : desc_kmajor(smem_base + kABytes);
-            const uint64_t a_lo0 = A_MN ? desc_mnmajor(smem_base + kLoBase) : desc_kmajor(smem_base + kLoBase);
-            const uint64_t b_lo0 = B_MN ? desc_mnmajor(smem_base + kLoBase + kABytes) : desc_kmajor(smem_base + kLoBase + kABytes);
-            constexpr uint64_t kStageInc = (uint64_t)(kRawStage >> 4);
-            constexpr uint64_t kAdvA = (uint64_t)((A_MN ? 1024 : 32) >> 4), kAdvB = (uint64_t)((B_MN ? 1024 : 32) >> 4);
-            const uint32_t acc_x = tmem_d + 3u * BN;
-            const bool full3 = grp.dbg_mode != 2;
-            int sr = 0, sl = 0;
-            uint32_t lpar = 0;
-#define SS_STEP(KK, ACC, FIRSTMAIN, FIRSTX)                                                                              \
-    if (full3) {                                                                                                         \
-        umma_tf32(acc_x, a_lo + (KK) * kAdvA, b_raw + (KK) * kAdvB, idesc, (FIRSTX) ? 0u : 1u);                          \
-        umma_tf32(acc_x, a_raw + (KK) * kAdvA, b_lo + (KK) * kAdvB, idesc, 1u);                                          \
-    }                                                                                                                    \
-    umma_tf32(tmem_d + (uint32_t)(ACC) * BN, a_raw + (KK) * kAdvA, b_raw + (KK) * kAdvB, idesc, (FIRSTMAIN) ? 0u : 1u);
-#define SS_BLOCK(FIRST)                                                                                                  \
-    {                                                                                                                    \
-        mbar_wait_spin(&lo_full[sl], (lpar >> sl) & 1u);     /* implies tma_full[sr] (the residual warps waited on it) */  \
-        lpar ^= 1u << sl;                                                                                                \
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");                                                  \
-        const uint64_t a_raw = a_raw0 + (uint64_t)sr * kStageInc, b_raw = b_raw0 + (uint64_t)sr * kStageInc;             \
-        const uint64_t a_lo = a_lo0 + (uint64_t)sl * kStageInc, b_lo = b_lo0 + (uint64_t)sl * kStageInc;                 \
-        SS_STEP(0, 0, FIRST, FIRST) SS_STEP(1, 1, FIRST, false) SS_STEP(2, 2, FIRST, false) SS_STEP(3, 0, false, false)  \
-        umma_commit(&raw_empty[sr]);                         /* both slots are free once these MMAs retire */            \
-        umma_commit(&lo_empty[sl]);                                                                                      \
-    }
-            if (nkb > 0) {
-                SS_BLOCK(true)
-                if (tr) tr_s[7] = gtimer();
-                sr = 1 % NR; sl = 1 % NL;
-                for (int kb = 1; kb < nkb; ++kb) {
-                    SS_BLOCK(false)
-                    sr = (sr + 1 == NR) ? 0 : sr + 1;
-                    sl = (sl + 1 == NL) ? 0 : sl + 1;
-                }
-            }
-#undef SS_BLOCK
-#undef SS_STEP
-            umma_commit(&accum_bar);
-            if (tr) tr_s[8] = gtimer();
-        }
-        __syncwarp();
-        // ===================== epilogue (warps 8-11 <-> TMEM lanes 32q..32q+31) =====================
-        const int q = warp - 8;
-        const int i = m0 + q * 32 + lane;
-        float* __restrict__ C = P.C + (long long)batch * P.sC + (long long)split * P.strideP;
-        const bool add_bias = (P.bias != nullptr) && (split == 0);
-        if (nkb > 0) {
-            mbar_wait(&accum_bar, 0);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        }
-        if (tr && warp == 10 && lane == 0) tr_s[9] = gtimer();
-        pdl_wait();                     // C may still be read (or accumulated into) by the predecessor
-        if (tr && warp == 10 && lane == 0) tr_s[12] = gtimer();
-        // every field of P used below is copied to a local first: P lives in the kernel parameter space behind a
-        // runtime group index, and the unrolled store loop would otherwise re-fetch it per element
-        const int Ma = P.Ma, Nb = P.Nb;
-        const long long c_rs = P.c_rs, c_cs = P.c_cs;
-        const bool accumulate = P.accumulate != 0;
-        const float* bias_n = (add_bias && !P.bias_on_a) ? P.bias : nullptr;
-        const float bias_a = (add_bias && P.bias_on_a && i < Ma) ? __ldg(P.bias + i) : 0.f;
-        const int dbg = grp.dbg_mode;
-        const bool c_vec_ok = (c_cs == 1) && ((c_rs & 3) == 0) && ((reinterpret_cast<uintptr_t>(C) & 15) == 0);
-#pragma unroll 1
-        for (int c0 = 0; c0 < BN; c0 += 32) {
-            if (n0 + c0 >= Nb) break;
-            // 32 columns per round: the eight TMEM loads (4 accumulators x 2 halves) are all in flight before the one wait
-            float r[32];
-            if (nkb > 0 && dbg != 4) {
-                uint32_t t0[16], t1[16], t2[16], t3[16], u0[16], u1[16], u2[16], u3[16];
-                const uint32_t ta = tmem_d + ((uint32_t)(q * 32) << 16) + (uint32_t)c0;
-                tmem_ld16(ta, t0);
-                tmem_ld16(ta + BN, t1);
-                tmem_ld16(ta + 2 * BN, t2);
-                tmem_ld16(ta + 3 * BN, t3);
-                tmem_ld16(ta + 16, u0);
-                tmem_ld16(ta + 16 + BN, u1);
-                tmem_ld16(ta + 16 + 2 * BN, u2);
-                tmem_ld16(ta + 16 + 3 * BN, u3);
-                asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-                if (tr && warp == 10 && lane == 0) tr_s[11] = gtimer();
-#pragma unroll
-                for (int t = 0; t < 16; ++t) {
-                    r[t] = ((__uint_as_float(t0[t]) + __uint_as_float(t1[t])) + __uint_as_float(t2[t])) + __uint_as_float(t3[t]) + bias_a;
-                    r[16 + t] = ((__uint_as_float(u0[t]) + __uint_as_float(u1[t])) + __uint_as_float(u2[t])) + __uint_as_float(u3[t]) + bias_a;
-                }
-            } else {
-#pragma unroll
-                for (int t = 0; t < 32; ++t) r[t] = bias_a;
-            }
-            if (i < Ma && dbg != 3) {
-                const int jb = n0 + c0;
-                const bool full = jb + 31 < Nb;
-                float* cp = C + (long long)i * c_rs + (long long)jb * c_cs;
-                if (full && !accumulate && bias_n == nullptr) {
-                    // the common case (split-K slabs, activations without a column bias): straight stores
-                    if (c_vec_ok) {
-#pragma unroll
-                        for (int t = 0; t < 32; t += 4)
-                            *reinterpret_cast<float4*>(cp + t) = make_float4(r[t], r[t + 1], r[t + 2], r[t + 3]);
-                    } else {
-#pragma unroll
-                        for (int t = 0; t < 32; ++t) cp[(long long)t * c_cs] = r[t];
-                    }
-                } else if (full && c_vec_ok) {
-#pragma unroll
-                    for (int t = 0; t < 32; t += 4) {
-                        float4 o = make_float4(r[t], r[t + 1], r[t + 2], r[t + 3]);
-                        if (bias_n) {
-                            o.x += __ldg(bias_n + jb + t); o.y += __ldg(bias_n + jb + t + 1);
-                            o.z += __ldg(bias_n + jb + t + 2); o.w += __ldg(bias_n + jb + t + 3);
-                        }
-                        float4* c4 = reinterpret_cast<float4*>(cp + t);
-                        if (accumulate) {
-                            const float4 old = *c4;
-                            o.x += old.x; o.y += old.y; o.z += old.z; o.w += old.w;
-                        }
-                        *c4 = o;
-                    }
-                } else {
-#pragma unroll 4
-                    for (int t = 0; t < 32; ++t) {
-                        if (jb + t < Nb) {
-                            float o = r[t];
-                            if (bias_n) o += __ldg(bias_n + jb + t);
-                            float* ce = cp + (long long)t * c_cs;
-                            if (accumulate) o += *ce;
-                            *ce = o;
-                        }
-                    }
-                }
-            }
-        }
-    }
-    if (tr && warp == 10 && lane == 0) tr_s[10] = gtimer();
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-#ifdef NATS_TRACE_BUILD
-    if (tr && tid == 0) {
-        const unsigned long long t0 = tr_s[0];
-        printf("[trace gemm BN=%d nkb=%d] start %llu | setup +%llu | prod: prewait +%llu wait_done +%llu issued +%llu | resid: first_full +%llu done +%llu | mma: first +%llu last_commit +%llu | epi: accum +%llu pdlwait +%llu tmem_ld +%llu stored +%llu | end +%llu ns\n",
-               BN, nkb, t0 % 100000000ull, tr_s[1] - t0, tr_s[2] - t0, tr_s[3] - t0, tr_s[4] - t0, tr_s[5] - t0, tr_s[6] - t0, tr_s[7] - t0,
-               tr_s[8] - t0, tr_s[9] - t0, tr_s[12] - t0, tr_s[11] - t0, tr_s[10] - t0, gtimer() - t0);
-    }
-#endif
-    if (warp == 8) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_d), "r"(kTmemCols) : "memory");
-    }
-}
-
-// ------------------------------------------------------------------------------------------------------------
-// TS variant for the skinny products (BN <= 64): the 128-row operand (the weights) is fed to the tensor core from
-// TENSOR MEMORY instead of shared memory.  The SS kernel above moves ~120 KB through the 128 B/clk shared-memory port
-// per 16 KB weight tile (TMA write, residual read+write, three UMMA operand reads) and is bound by it; here the eight
-// split warps read the raw tile ONCE and write both halves  hi = trunc_tf32(x),  lo = x - hi  into TMEM with
-// tcgen05.st (lane = row m, column = k), and the three MMAs of a k-step read A from TMEM: 56 KB per tile.
-//   raw stage (shared, NR deep): [A_raw 16 KB | B_raw | B_lo]      A stage (TMEM, NL deep): [hi 32 cols | lo 32 cols]
-template <int BN, int NR, int NL, bool A_MN, bool B_MN>
-__global__ void __launch_bounds__(kThreads, 1) tma_gemm_ts_kernel(const __grid_constant__ TmaGroup grp) {
-    constexpr uint32_t kABytes = 128 * 128, kBBytes = BN * 128;
-    constexpr uint32_t kRawStage = kABytes + 2 * kBBytes;
-    // accumulators: NACC rotating [hi*hi | hi*lo] pairs (2*BN columns each, one N-stacked MMA) + one lo*hi (BN columns).
-    // The tensor core spends the same ~69 cycles on an M128 x N<=128 x K8 step whatever N is, so stacking the two
-    // products that share A_hi along N turns three MMAs per k-step into two.
-    constexpr uint32_t NACC = BN <= 32 ? 3 : 2;
-    constexpr uint32_t kAccCols = NACC * 2 * BN + BN;
-    constexpr uint32_t kTmemCols = (kAccCols + NL * 64 <= 128) ? 128 : ((kAccCols + NL * 64 <= 256) ? 256 : 512);
-    static_assert(kAccCols + NL * 64 <= 512, "tensor memory budget");
-
-    extern __shared__ __align__(1024) unsigned char smem[];
-    __shared__ __align__(8) uint64_t tma_full[NR];
-    // One tcgen05.commit per TWO k-blocks (a commit costs the issuing thread ~120 cycles, an MMA ~50): k-block j is known to
-    // have retired when barrier done[(j|1) % NR] completes its ((j|1) / NR)-th phase.  Both the TMA producer (shared stage
-    // j % NR is free) and the split warps (tensor-memory stage j % NL is free) wait on it.
-    static_assert(NR % 2 == 0 && NL <= NR, "ring depths");
-    __shared__ __align__(8) uint64_t done[NR];
-    __shared__ __align__(8) uint64_t a_full[NL];
-    __shared__ __align__(8) uint64_t accum_bar;
-    __shared__ uint32_t tmem_base_slot;
-    __shared__ unsigned long long tr_s[16];
-#ifdef NATS_TRACE_BUILD
-    const bool tr = grp.trace && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0;
-#else
-    constexpr bool tr = false;
-#endif
-    if (tr && threadIdx.x == 0) tr_s[0] = gtimer();
-
-    int z = blockIdx.z, g = 0;
-    if (grp.count > 1 && z >= grp.zstart[1]) g = 1;
-    const TmaProblem& P = grp.p[g];
-    const CUtensorMap* mapA = &grp.mapA[g];
-    const CUtensorMap* mapB = &grp.mapB[g];
-    z -= grp.zstart[g];
-    const int split = z % P.splitk, batch = z / P.splitk;
-    const int m0 = blockIdx.x * 128, n0 = blockIdx.y * BN;
-    if (m0 >= P.Ma || n0 >= P.Nb) return;
-
-    const int kbeg = split * P.kchunk;
-    const int kend = min(P.K, kbeg + P.kchunk);
-    const int nkb = (kend > kbeg) ? (kend - kbeg + kBlockK - 1) / kBlockK : 0;
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const uint32_t smem_base = (smem_u32(smem) + 1023u) & ~1023u;
-
-    if (tid == 0) {
-        asm volatile("prefetch.tensormap [%0];" ::"l"(mapA) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(mapB) : "memory");
-        for (int s = 0; s < NR; ++s) { mbar_init(&tma_full[s], 1); mbar_init(&done[s], 1); }
-        for (int s = 0; s < NL; ++s) mbar_init(&a_full[s], kSplitThreads / 32);
-        mbar_init(&accum_bar, 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 8) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_base_slot)),
-                     "r"(kTmemCols)
-                     : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_d = tmem_base_slot;
-    const uint32_t tmem_a0 = tmem_d + kAccCols;
-    if (tr && tid == 0) tr_s[1] = gtimer();
-    pdl_trigger();
-    const int npre_w = P.a_static ? min(nkb, NR) : 0;      // weight tiles requested before any dependency wait
-    if (warp == 8 && lane == 0) {
-        for (int kb = 0; kb < npre_w; ++kb) {
-            const uint32_t raw = smem_base + (uint32_t)kb * kRawStage;
-            const int k0 = kbeg + kb * kBlockK;
-            mbar_expect_tx_only(&tma_full[kb], kABytes);
-            if (A_MN) {
-#pragma unroll
-                for (int bi = 0; bi < 4; ++bi) tma_load_3d(raw + bi * 4096, mapA, &tma_full[kb], m0 + 32 * bi, k0, batch);
-            } else {
-                tma_load_3d(raw, mapA, &tma_full[kb], k0, m0, batch);
-            }
-        }
-    }
-
-    if (warp < 8) {
-        // ===================== split pass: raw A tile -> (hi, lo) in tensor memory; raw B tile -> B_lo in shared =====
-        const int q = warp & 3, h = warp >> 2;          // TMEM lane quadrant of this warp / which 16 of the 32 k
-        const int m = 32 * q + lane;                    // row of the 128-row tile handled by this thread
-        for (int kb = 0; kb < nkb; ++kb) {
-            const int sr = kb % NR, sl = kb % NL;
-            if (kb >= NL) {                                                 // the MMAs that read this TMEM stage retired
-                const int c = (kb - NL) | 1;
-                mbar_wait(&done[c % NR], (uint32_t)((c / NR) & 1));
-            }
-            mbar_wait(&tma_full[sr], (uint32_t)((kb / NR) & 1));            // raw tiles landed
-            if (tr && tid == 0 && kb == 0) tr_s[5] = gtimer();
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            const uint32_t raw = smem_base + (uint32_t)sr * kRawStage;
-            float v[16];
-            if (!A_MN) {        // K-major: row m = 128 B, 16-byte chunks XOR (m & 7)
-#pragma unroll
-                for (int c = 0; c < 4; ++c) {
-                    const uint32_t addr = raw + (uint32_t)m * 128u + (uint32_t)((((4 * h + c) ^ (m & 7))) << 4);
-                    asm volatile("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];"
-                                 : "=f"(v[4 * c]), "=f"(v[4 * c + 1]), "=f"(v[4 * c + 2]), "=f"(v[4 * c + 3])
-                                 : "r"(addr));
-                }
-            } else {            // MN-major (SW128_32B): 32-row blocks of 4096 B, k rows of 128 B, 32-byte chunks XOR (k & 3)
-#pragma unroll
-                for (int j = 0; j < 16; ++j) {
-                    const int k = 16 * h + j;
-                    const uint32_t addr = raw + (uint32_t)(m >> 5) * 4096u + (uint32_t)k * 128u +
-                                          (uint32_t)(((((m & 31) >> 3) ^ (k & 3))) << 5) + (uint32_t)((m & 7) << 2);
-                    asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v[j]) : "r"(addr));
-                }
-            }
-            uint32_t hi[16], lo[16];
-#pragma unroll
-            for (int j = 0; j < 16; ++j) {
-                hi[j] = __float_as_uint(v[j]) & 0xFFFFE000u;
-                lo[j] = __float_as_uint(v[j] - __uint_as_float(hi[j]));
-            }
-            const uint32_t ta = tmem_a0 + ((uint32_t)(32 * q) << 16) + (uint32_t)(sl * 64 + 16 * h);
-            tmem_st16(ta, hi);
-            tmem_st16(ta + 32, lo);
-            // B: lo = raw - trunc(raw), same stage, next to the raw tile
-#pragma unroll
-            for (int i = 0; i < (int)(kBBytes / 16 + kSplitThreads - 1) / kSplitThreads; ++i) {
-                const uint32_t e = (uint32_t)(tid + i * kSplitThreads);
-                if (e < kBBytes / 16) {
-                    float4 b;
-                    asm volatile("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(b.x), "=f"(b.y), "=f"(b.z), "=f"(b.w) : "r"(raw + kABytes + e * 16u));
-                    asm volatile("st.shared.v4.f32 [%0], {%1,%2,%3,%4};" ::"r"(raw + kABytes + kBBytes + e * 16u), "f"(resid(b.x)),
-                                 "f"(resid(b.y)), "f"(resid(b.z)), "f"(resid(b.w))
-                                 : "memory");
-                }
-            }
-            asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-            asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&a_full[sl]);
-            if (tr && tid == 0 && kb == 0) tr_s[13] = gtimer();
-        }
-        if (tr && tid == 0) tr_s[6] = gtimer();
-    } else {
-        if (warp == 8 && lane == 0) {
-            // ===================== TMA producer (as in the SS kernel) =====================
-            const int npre = npre_w;
-            if (tr) tr_s[2] = gtimer();
-            pdl_wait();
-            if (tr) tr_s[3] = gtimer();
-            for (int kb = 0; kb < nkb; ++kb) {
-                const int sr = kb % NR;
-                if (kb >= NR) {
-                    const int c = (kb - NR) | 1;
-                    mbar_wait(&done[c % NR], (uint32_t)((c / NR) & 1));
-                }
-                const uint32_t raw = smem_base + (uint32_t)sr * kRawStage;
-                const int k0 = kbeg + kb * kBlockK;
-                if (kb < npre) {
-                    mbar_expect_tx(&tma_full[sr], kBBytes);
-                } else {
-                    mbar_expect_tx(&tma_full[sr], kABytes + kBBytes);
-                    if (A_MN) {
-#pragma unroll
-                        for (int bi = 0; bi < 4; ++bi) tma_load_3d(raw + bi * 4096, mapA, &tma_full[sr], m0 + 32 * bi, k0, batch);
-                    } else {
-                        tma_load_3d(raw, mapA, &tma_full[sr], k0, m0, batch);
-                    }
-                }
-                if (B_MN) {
-#pragma unroll
-                    for (int bi = 0; bi < BN / 32; ++bi)
-                        tma_load_3d(raw + kABytes + bi * 4096, mapB, &tma_full[sr], n0 + 32 * bi, k0, batch);
-                } else {
-                    tma_load_3d(raw + kABytes, mapB, &tma_full[sr], k0, n0, batch);
-                }
-            }
-        } else if (warp == 9 && lane == 0) {
-            // ===================== MMA issuer: A from tensor memory (always K-major there), B from shared =============
-            const uint32_t idesc_base = (1u << 4) | (2u << 7) | (2u << 10) | ((B_MN ? 1u : 0u) << 16) | ((128u >> 4) << 24);
-            const uint32_t idesc1 = idesc_base | ((uint32_t)(BN >> 3) << 17);            // N = BN
-            const uint32_t idesc2 = idesc_base | ((uint32_t)((2 * BN) >> 3) << 17);      // N = 2*BN: [B_raw | B_lo]
-            // Straight-line issue code (see enc_tc.cu): a single thread executes dependent scalar instructions at ~10 cycles
-            // each, so runtime accumulate predicates, modulo rotations and descriptor rebuilds between two MMAs cost more
-            // than the MMAs.  The first k-block is peeled (its MMAs overwrite the accumulators), the accumulator of a k-step
-            // is fixed by its position in the block (kk % NACC), ring indices are running counters.
-            const uint64_t b_desc0 = B_MN ? desc_mnmajor(smem_base + kABytes) : desc_kmajor(smem_base + kABytes);   // B_lo follows contiguously
-            constexpr uint64_t kStageInc = (uint64_t)(kRawStage >> 4);
-            constexpr uint64_t kAdv = (uint64_t)((B_MN ? 1024 : 32) >> 4);
-            const uint32_t acc_lo = tmem_d + NACC * 2u * BN;
-            int sr = 0, sl = 0;
-            uint32_t apar = 0;                               // parity bit per TMEM stage
-#define TS_BLOCK(FIRST)                                                                                                   \
-    {                                                                                                                     \
-        mbar_wait_spin(&a_full[sl], (apar >> sl) & 1u);                                                                   \
-        apar ^= 1u << sl;                                                                                                 \
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");                                                   \
-        const uint64_t b_raw = b_desc0 + (uint64_t)sr * kStageInc;                                                        \
-        const uint32_t a_hi = tmem_a0 + (uint32_t)(sl * 64), a_lo = a_hi + 32;                                            \
-        umma_tf32_ts(acc_lo, a_lo, b_raw, idesc1, (FIRST) ? 0u : 1u);                                                     \
-        umma_tf32_ts(tmem_d, a_hi, b_raw, idesc2, (FIRST) ? 0u : 1u);                                                     \
-        umma_tf32_ts(acc_lo, a_lo + 8u, b_raw + kAdv, idesc1, 1u);                                                        \
-        umma_tf32_ts(tmem_d + 2u * BN, a_hi + 8u, b_raw + kAdv, idesc2, (FIRST) ? 0u : 1u);                               \
-        umma_tf32_ts(acc_lo, a_lo + 16u, b_raw + 2 * kAdv, idesc1, 1u);                                                   \
-        umma_tf32_ts(tmem_d + (NACC > 2 ? 4u * BN : 0u), a_hi + 16u, b_raw + 2 * kAdv, idesc2, (FIRST) && NACC > 2 ? 0u : 1u); \
-        umma_tf32_ts(acc_lo, a_lo + 24u, b_raw + 3 * kAdv, idesc1, 1u);                                                   \
-        umma_tf32_ts(tmem_d + (NACC > 2 ? 0u : 2u * BN), a_hi + 24u, b_raw + 3 * kAdv, idesc2, 1u);                       \
-    }
-            if (nkb > 0) {
-                TS_BLOCK(true)
-                if (tr) tr_s[7] = gtimer();
-                sr = 1; sl = 1 % NL;
-                for (int kb = 1; kb < nkb; ++kb) {
-                    TS_BLOCK(false)
-                    if (kb & 1) umma_commit(&done[sr]);
-                    sr = (sr + 1 == NR) ? 0 : sr + 1;
-                    sl = (sl + 1 == NL) ? 0 : sl + 1;
-                }
-            }
-#undef TS_BLOCK
-            umma_commit(&accum_bar);
-            if (tr) tr_s[8] = gtimer();
-        }
-        __syncwarp();
-        // ===================== epilogue (identical to the SS kernel) =====================
-        const int q = warp - 8;
-        const int i = m0 + q * 32 + lane;
-        float* __restrict__ C = P.C + (long long)batch * P.sC + (long long)split * P.strideP;
-        const bool add_bias = (P.bias != nullptr) && (split == 0);
-        if (nkb > 0) {
-            mbar_wait(&accum_bar, 0);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        }
-        if (tr && warp == 10 && lane == 0) tr_s[9] = gtimer();
-        pdl_wait();
-        const int Ma = P.Ma, Nb = P.Nb;
-        const long long c_rs = P.c_rs, c_cs = P.c_cs;
-        const bool accumulate = P.accumulate != 0;
-        const float* bias_n = (add_bias && !P.bias_on_a) ? P.bias : nullptr;
-        const float bias_a = (add_bias && P.bias_on_a && i < Ma) ? __ldg(P.bias + i) : 0.f;
-        const bool c_vec_ok = (c_cs == 1) && ((c_rs & 3) == 0) && ((reinterpret_cast<uintptr_t>(C) & 15) == 0);
-#pragma unroll 1
-        for (int c0 = 0; c0 < BN; c0 += 32) {
-            if (n0 + c0 >= Nb) break;
-            float r[32];
-            if (nkb > 0) {
-#pragma unroll
-                for (int hh = 0; hh < 2; ++hh) {            // 16 columns at a time: 2*NACC + 1 TMEM loads in flight
-                    uint32_t t[2 * NACC + 1][16];
-                    const uint32_t ta = tmem_d + ((uint32_t)(q * 32) << 16) + (uint32_t)(c0 + 16 * hh);
-#pragma unroll
-                    for (int a = 0; a < (int)NACC; ++a) {
-                        tmem_ld16(ta + a * 2 * BN, t[2 * a]);              // hi*hi
-                        tmem_ld16(ta + a * 2 * BN + BN, t[2 * a + 1]);     // hi*lo
-                    }
-                    tmem_ld16(ta + NACC * 2 * BN, t[2 * NACC]);            // lo*hi
-                    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-                    for (int e = 0; e < 16; ++e) {
-                        float main_sum = __uint_as_float(t[0][e]);
-#pragma unroll
-                        for (int a = 1; a < (int)NACC; ++a) main_sum += __uint_as_float(t[2 * a][e]);
-                        float cross = __uint_as_float(t[2 * NACC][e]);
-#pragma unroll
-                        for (int a = 0; a < (int)NACC; ++a) cross += __uint_as_float(t[2 * a + 1][e]);
-                        r[16 * hh + e] = (main_sum + cross) + bias_a;
-                    }
-                }
-            } else {
-#pragma unroll
-                for (int t = 0; t < 32; ++t) r[t] = bias_a;
-            }
-            if (i < Ma) {
-                const int jb = n0 + c0;
-                const bool full = jb + 31 < Nb;
-                float* cp = C + (long long)i * c_rs + (long long)jb * c_cs;
-                if (full && !accumulate && bias_n == nullptr) {
-                    if (c_vec_ok) {
-#pragma unroll
-                        for (int t = 0; t < 32; t += 4)
-                            *reinterpret_cast<float4*>(cp + t) = make_float4(r[t], r[t + 1], r[t + 2], r[t + 3]);
-                    } else {
-#pragma unroll
-                        for (int t = 0; t < 32; ++t) cp[(long long)t * c_cs] = r[t];
-                    }
-                } else {
-#pragma unroll 4
-                    for (int t = 0; t < 32; ++t) {
-                        if (jb + t < Nb) {
-                            float o = r[t];
-                            if (bias_n) o += __ldg(bias_n + jb + t);
-                            float* ce = cp + (long long)t * c_cs;
-                            if (accumulate) o += *ce;
-                            *ce = o;
-                        }
-                    }
-                }
-            }
-        }
-    }
-    if (tr && warp == 10 && lane == 0) tr_s[10] = gtimer();
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-#ifdef NATS_TRACE_BUILD
-    if (tr && tid == 0) {
-        const unsigned long long t0 = tr_s[0];
-        printf("[trace ts-gemm BN=%d nkb=%d] start %llu | setup +%llu | prod: prewait +%llu wait_done +%llu | split: first_full +%llu first_done +%llu all_done +%llu | mma: first +%llu last_commit +%llu | epi: accum +%llu stored +%llu | end +%llu ns\n",
-               BN, nkb, t0 % 100000000ull, tr_s[1] - t0, tr_s[2] - t0, tr_s[3] - t0, tr_s[5] - t0, tr_s[13] - t0, tr_s[6] - t0, tr_s[7] - t0,
-               tr_s[8] - t0, tr_s[9] - t0, tr_s[10] - t0, gtimer() - t0);
-    }
-#endif
-    if (warp == 8) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_d), "r"(kTmemCols) : "memory");
-    }
-}
-
-template <int BN, int NR>
-constexpr size_t ts_smem_bytes() { return (size_t)NR * (128 * 128 + 2 * BN * 128) + 1024; }
-
-template <int BN, int NR, int NL>
-constexpr size_t smem_bytes() { return (size_t)(NR + NL) * (128 * 128 + BN * 128) + 1024; }
-
-// ------------------------------------------------------------------ host: tensor maps
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -710,93 +44,245 @@ struct MapKeyHash {
 };
 std::unordered_map<MapKey, CUtensorMap, MapKeyHash> g_maps;
 
-// 3-D map over a (batch, outer, inner) fp32 array; box = (1, box_outer, 32 floats = one 128-byte swizzle row)
-int get_map(const float* ptr, long long inner, long long outer, long long ld, long long batch, long long bstride,
-            int box_outer, bool mn_major, CUtensorMap* out) {
-    MapKey key{ptr, inner, outer, ld, batch, bstride, box_outer, mn_major ? 1 : 0};
-    auto it = g_maps.find(key);
-    if (it != g_maps.end()) { *out = it->second; return 0; }
-    if (g_maps.size() > (1u << 16)) g_maps.clear();
-    cuuint64_t gdim[3] = {(cuuint64_t)inner, (cuuint64_t)outer, (cuuint64_t)(batch < 1 ? 1 : batch)};
-    cuuint64_t gstr[2] = {(cuuint64_t)ld * 4, (cuuint64_t)(batch > 1 ? bstride : (long long)outer * ld) * 4};
-    if (gstr[1] == 0) gstr[1] = 16;
-    cuuint32_t box[3] = {32, (cuuint32_t)box_outer, 1};
-    cuuint32_t estr[3] = {1, 1, 1};
-    CUtensorMap m;
-    const CUresult r = g_encode(&m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(ptr), gdim, gstr, box, estr,
-                                CU_TENSOR_MAP_INTERLEAVE_NONE,
-                                mn_major ? CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B : CU_TENSOR_MAP_SWIZZLE_128B,
-                                CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) {
-        set_error("cuTensorMapEncodeTiled failed (%d): ptr=%p inner=%lld outer=%lld ld=%lld batch=%lld", (int)r, ptr, inner,
-                  outer, ld, batch);
-        return 1;
-    }
-    g_maps.emplace(key, m);
-    *out = m;
-    return 0;
+
+constexpr int kThreads = 256;
+constexpr int kBlockK = 32;
+constexpr int kNR = 3;                  // raw stages in flight
+constexpr int kMaxGroup = 2;
+
+struct TmaProblem {
+    float* C;
+    const float* bias;
+    int Ma, Nb, K;
+    long long c_rs, c_cs;
+    int batch;
+    long long sC;
+    int splitk, kchunk;
+    long long strideP;
+    int accumulate;
+    int bias_on_a;
+};
+struct alignas(64) TmaGroup {
+    CUtensorMap mapA[kMaxGroup];
+    CUtensorMap mapB[kMaxGroup];
+    TmaProblem p[kMaxGroup];
+    int zstart[kMaxGroup + 1];
+    int count;
+};
+
+using namespace tc;
+
+// raw stage of an operand: ROWS x 32 fp32 as TMA wrote it: K-major [ROWS][32] or MN-major [32][ROWS] (unswizzled)
+template <int ROWS, bool MN>
+__device__ __forceinline__ float raw_at(uint32_t raw, int r, int k) {
+    float v;
+    asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(raw + 4u * (uint32_t)(MN ? k * ROWS + r : r * 32 + k)));
+    return v;
 }
 
-static int g_trace_on = 0;
-static int g_ts_mode = 1;        // 1: skinny products (BN <= 64) read the 128-row operand from tensor memory
-static int g_dbg_mode = 0;
-static long long g_trace_no = 0;
-
-template <int BN, int NR, int NL>
-int launch_bn(cudaStream_t st, TmaGroup& grp, bool a_mn, bool b_mn, dim3 grid, double flops, double bytes) {
-    grp.dbg_mode = g_dbg_mode;
-    if (g_trace_on && BN == 32) {
-        ++g_trace_no;
-        grp.trace = (g_trace_no >= g_trace_on && g_trace_no < g_trace_on + 4) ? 1 : 0;
-    }
-    ProfScope ps(st, BN <= 64 ? K_TC_GEMM_SKINNY : K_TC_GEMM, flops, bytes);
-    if constexpr (BN <= 64) {
-        if (g_ts_mode) {
-            constexpr int TNR = BN == 32 ? 8 : 6, TNL = BN == 32 ? 4 : 3;
-            const size_t tsm = ts_smem_bytes<BN, TNR>();
-            cudaError_t e;
-            if (!a_mn && !b_mn) e = launch_pdl(tma_gemm_ts_kernel<BN, TNR, TNL, false, false>, grid, dim3(kThreads), tsm, st, grp);
-            else if (!a_mn && b_mn) e = launch_pdl(tma_gemm_ts_kernel<BN, TNR, TNL, false, true>, grid, dim3(kThreads), tsm, st, grp);
-            else if (a_mn && !b_mn) e = launch_pdl(tma_gemm_ts_kernel<BN, TNR, TNL, true, false>, grid, dim3(kThreads), tsm, st, grp);
-            else e = launch_pdl(tma_gemm_ts_kernel<BN, TNR, TNL, true, true>, grid, dim3(kThreads), tsm, st, grp);
-            NATS_CUDA_OK(e);
-            return 0;
+// raw stage -> {hi, lo} K-major SWIZZLE_128B tiles (16-byte chunk c of row r at chunk c ^ (r & 7)); k >= klim reads as 0
+template <int ROWS, bool MN>
+__device__ __forceinline__ void split_tile(uint32_t raw, uint32_t hi_base, uint32_t lo_base, int klim, int tid) {
+    constexpr int kChunks = ROWS * 8;
+#pragma unroll
+    for (int i = 0; i < (kChunks + kThreads - 1) / kThreads; ++i) {
+        const int q = tid + i * kThreads;
+        if (q < kChunks) {
+            int r, c;
+            float4 v;
+            if (!MN) {
+                r = q >> 3; c = q & 7;
+                asm volatile("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w)
+                             : "r"(raw + 4u * (uint32_t)(r * 32 + 4 * c)));
+            } else {                                          // a warp covers 32 consecutive rows: conflict-free reads
+                r = q % ROWS; c = q / ROWS;
+                v.x = raw_at<ROWS, true>(raw, r, 4 * c); v.y = raw_at<ROWS, true>(raw, r, 4 * c + 1);
+                v.z = raw_at<ROWS, true>(raw, r, 4 * c + 2); v.w = raw_at<ROWS, true>(raw, r, 4 * c + 3);
+            }
+            if (4 * c >= klim) v.x = 0.f;
+            if (4 * c + 1 >= klim) v.y = 0.f;
+            if (4 * c + 2 >= klim) v.z = 0.f;
+            if (4 * c + 3 >= klim) v.w = 0.f;
+            float4 hi, lo;
+            hi.x = to_tf32(v.x); hi.y = to_tf32(v.y); hi.z = to_tf32(v.z); hi.w = to_tf32(v.w);
+            lo.x = to_tf32(v.x - hi.x); lo.y = to_tf32(v.y - hi.y); lo.z = to_tf32(v.z - hi.z); lo.w = to_tf32(v.w - hi.w);
+            const uint32_t off = (uint32_t)(r * 128 + ((c ^ (r & 7)) << 4));
+            st_shared_v4(hi_base + off, hi);
+            st_shared_v4(lo_base + off, lo);
         }
     }
-    const size_t sm = smem_bytes<BN, NR, NL>();
-    cudaError_t le;
-    if (!a_mn && !b_mn) le = launch_pdl(tma_gemm_kernel<BN, NR, NL, false, false>, grid, dim3(kThreads), sm, st, grp);
-    else if (!a_mn && b_mn) le = launch_pdl(tma_gemm_kernel<BN, NR, NL, false, true>, grid, dim3(kThreads), sm, st, grp);
-    else if (a_mn && !b_mn) le = launch_pdl(tma_gemm_kernel<BN, NR, NL, true, false>, grid, dim3(kThreads), sm, st, grp);
-    else le = launch_pdl(tma_gemm_kernel<BN, NR, NL, true, true>, grid, dim3(kThreads), sm, st, grp);
-    NATS_CUDA_OK(le);
+}
+
+template <int BN>
+__device__ __forceinline__ void mma_ss(float (&d)[BN / 2], uint64_t da, uint64_t db) {
+    if constexpr (BN == 32) wgmma_ss_n32(d, da, db);
+    else wgmma_ss_n64(d, da, db);
+}
+template <int BN>
+__device__ __forceinline__ void mma_rs(float (&d)[BN / 2], const uint32_t (&a)[4], uint64_t db) {
+    if constexpr (BN == 32) wgmma_rs_n32(d, a, db);
+    else wgmma_rs_n64(d, a, db);
+}
+
+template <int BN, bool A_MN, bool B_MN, bool A_REG>
+__global__ void __launch_bounds__(kThreads, 1) tma_gemm_kernel(const __grid_constant__ TmaGroup grp) {
+    constexpr uint32_t kARaw = 128 * 128, kBRaw = BN * 128;
+    constexpr uint32_t kRawStage = kARaw + kBRaw;
+    constexpr uint32_t kAHalf = A_REG ? 0 : 128 * 128;              // A hi / lo tiles (none when A goes through registers)
+    constexpr uint32_t kSplitStage = 2 * kAHalf + 2 * kBRaw;
+    constexpr uint32_t kSplitBase = kNR * kRawStage;
+    constexpr int R = BN / 2;
+    static_assert(BN == 32 || BN == 64, "BN");
+
+    extern __shared__ __align__(1024) unsigned char smem[];
+    __shared__ __align__(8) uint64_t full[kNR];
+
+    int z = blockIdx.z, g = 0;
+    if (grp.count > 1 && z >= grp.zstart[1]) g = 1;
+    const TmaProblem& P = grp.p[g];
+    const CUtensorMap* mapA = &grp.mapA[g];
+    const CUtensorMap* mapB = &grp.mapB[g];
+    z -= grp.zstart[g];
+    const int split = z % P.splitk, batch = z / P.splitk;
+    const int m0 = blockIdx.x * 128, n0 = blockIdx.y * BN;
+    if (m0 >= P.Ma || n0 >= P.Nb) return;
+
+    const int kbeg = split * P.kchunk;
+    const int kend = min(P.K, kbeg + P.kchunk);
+    const int nkb = (kend > kbeg) ? (kend - kbeg + kBlockK - 1) / kBlockK : 0;
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = tid >> 7;
+    const uint32_t smem_base = (smem_u32(smem) + 1023u) & ~1023u;
+
+    if (tid == 0) {
+        asm volatile("prefetch.tensormap [%0];" ::"l"(mapA) : "memory");
+        asm volatile("prefetch.tensormap [%0];" ::"l"(mapB) : "memory");
+        for (int s = 0; s < kNR; ++s) mbar_init(&full[s], 1);
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+    pdl_trigger();
+    pdl_wait();                          // operands and C may be written by the predecessor
+
+    auto issue = [&](int kb) {           // thread 0: raw boxes of k-block kb into stage kb % kNR
+        const int s = kb % kNR;
+        const uint32_t raw = smem_base + (uint32_t)s * kRawStage;
+        const int k0 = kbeg + kb * kBlockK;
+        mbar_expect_tx(&full[s], kRawStage);
+        if (A_MN) tma_load_3d(raw, mapA, &full[s], m0, k0, batch);
+        else tma_load_3d(raw, mapA, &full[s], k0, m0, batch);
+        if (B_MN) tma_load_3d(raw + kARaw, mapB, &full[s], n0, k0, batch);
+        else tma_load_3d(raw + kARaw, mapB, &full[s], k0, n0, batch);
+    };
+    auto split_stage = [&](int kb) {     // raw stage of k-block kb -> split buffer kb & 1
+        mbar_wait(&full[kb % kNR], (uint32_t)((kb / kNR) & 1));
+        const uint32_t raw = smem_base + (uint32_t)(kb % kNR) * kRawStage;
+        const uint32_t sp = smem_base + kSplitBase + (uint32_t)(kb & 1) * kSplitStage;
+        const int klim = kend - (kbeg + kb * kBlockK);
+        if (!A_REG) split_tile<128, A_MN>(raw, sp, sp + kAHalf, klim, tid);
+        split_tile<BN, B_MN>(raw + kARaw, sp + 2 * kAHalf, sp + 2 * kAHalf + kBRaw, klim, tid);
+    };
+
+    float acc0[R], acc1[R], accx[R];
+#pragma unroll
+    for (int i = 0; i < R; ++i) { acc0[i] = 0.f; acc1[i] = 0.f; accx[i] = 0.f; }
+    const int r0 = 64 * wg + 16 * (warp & 3) + (lane >> 2);     // A fragment rows r0, r0 + 8 (register form)
+    const int q = lane & 3;
+
+    if (nkb > 0) {
+        if (tid == 0)
+            for (int kb = 0; kb < min(nkb, kNR); ++kb) issue(kb);
+        split_stage(0);
+    }
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> async proxy (wgmma)
+    __syncthreads();
+    for (int kb = 0; kb < nkb; ++kb) {
+        const uint32_t sp = smem_base + kSplitBase + (uint32_t)(kb & 1) * kSplitStage;
+        const uint64_t b_hi = desc_sw128(sp + 2 * kAHalf), b_lo = desc_sw128(sp + 2 * kAHalf + kBRaw);
+        if constexpr (A_REG) {
+            // A fragments of the 4 k-steps from the raw stage (full[] of this stage was waited on by split_stage)
+            const uint32_t raw = smem_base + (uint32_t)(kb % kNR) * kRawStage;
+            const int klim = kend - (kbeg + kb * kBlockK);
+            uint32_t ahi[4][4], alo[4][4];
+#pragma unroll
+            for (int kk = 0; kk < 4; ++kk) {
+#pragma unroll
+                for (int f = 0; f < 4; ++f) {
+                    const int r = r0 + 8 * (f & 1), k = 8 * kk + q + 4 * (f >> 1);
+                    const float x = k < klim ? raw_at<128, A_MN>(raw, r, k) : 0.f;
+                    const float h = to_tf32(x);
+                    ahi[kk][f] = __float_as_uint(h);
+                    alo[kk][f] = __float_as_uint(to_tf32(x - h));
+                }
+            }
+            wgmma_fence();
+#pragma unroll
+            for (int kk = 0; kk < 4; ++kk) {
+                mma_rs<BN>(accx, alo[kk], b_hi + 2 * kk);
+                mma_rs<BN>(accx, ahi[kk], b_lo + 2 * kk);
+                mma_rs<BN>((kk & 1) ? acc1 : acc0, ahi[kk], b_hi + 2 * kk);
+            }
+        } else {
+            const uint64_t a_hi = desc_sw128(sp + (uint32_t)wg * 8192u), a_lo = desc_sw128(sp + kAHalf + (uint32_t)wg * 8192u);
+            wgmma_fence();
+#pragma unroll
+            for (int kk = 0; kk < 4; ++kk) {
+                mma_ss<BN>(accx, a_lo + 2 * kk, b_hi + 2 * kk);
+                mma_ss<BN>(accx, a_hi + 2 * kk, b_lo + 2 * kk);
+                mma_ss<BN>((kk & 1) ? acc1 : acc0, a_hi + 2 * kk, b_hi + 2 * kk);
+            }
+        }
+        wgmma_commit();
+        if (kb + 1 < nkb) split_stage(kb + 1);    // the other split buffer was drained by the wait of the previous k-block
+        wgmma_wait<0>();
+        reg_fence(acc0); reg_fence(acc1); reg_fence(accx);
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+        __syncthreads();                          // every thread is done with raw stage kb % kNR
+        if (tid == 0 && kb + kNR < nkb) issue(kb + kNR);
+    }
+
+    const bool add_bias = (P.bias != nullptr) && (split == 0);
+    gemm_epilogue(acc0, acc1, accx, P.C + (long long)batch * P.sC + (long long)split * P.strideP, P.c_rs, P.c_cs, P.Ma, P.Nb,
+                  m0 + r0, n0 + 2 * q, (add_bias && P.bias_on_a) ? P.bias : nullptr,
+                  (add_bias && !P.bias_on_a) ? P.bias : nullptr, P.accumulate != 0);
+}
+
+template <int BN, bool A_REG>
+constexpr size_t smem_bytes() {
+    return (size_t)kNR * (128 * 128 + BN * 128) + 2 * (size_t)(2 * (A_REG ? 0 : 128 * 128) + 2 * BN * 128) + 1024;
+}
+
+template <int BN, bool A_REG>
+int set_attrs() {
+    const int sm = (int)smem_bytes<BN, A_REG>();
+    NATS_CUDA_OK(cudaFuncSetAttribute(tma_gemm_kernel<BN, false, false, A_REG>, cudaFuncAttributeMaxDynamicSharedMemorySize, sm));
+    NATS_CUDA_OK(cudaFuncSetAttribute(tma_gemm_kernel<BN, false, true, A_REG>, cudaFuncAttributeMaxDynamicSharedMemorySize, sm));
+    NATS_CUDA_OK(cudaFuncSetAttribute(tma_gemm_kernel<BN, true, false, A_REG>, cudaFuncAttributeMaxDynamicSharedMemorySize, sm));
+    NATS_CUDA_OK(cudaFuncSetAttribute(tma_gemm_kernel<BN, true, true, A_REG>, cudaFuncAttributeMaxDynamicSharedMemorySize, sm));
     return 0;
 }
 
-template <int BN, int NR, int NL>
-int set_attrs() {
-    const int sm = (int)smem_bytes<BN, NR, NL>();
-    NATS_CUDA_OK(cudaFuncSetAttribute(tma_gemm_kernel<BN, NR, NL, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, sm));
-    NATS_CUDA_OK(cudaFuncSetAttribute(tma_gemm_kernel<BN, NR, NL, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, sm));
-    NATS_CUDA_OK(cudaFuncSetAttribute(tma_gemm_kernel<BN, NR, NL, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, sm));
-    NATS_CUDA_OK(cudaFuncSetAttribute(tma_gemm_kernel<BN, NR, NL, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, sm));
-    if constexpr (BN <= 64) {
-        constexpr int TNR = BN == 32 ? 8 : 6, TNL = BN == 32 ? 4 : 3;
-        const int tsm = (int)ts_smem_bytes<BN, TNR>();
-        NATS_CUDA_OK(cudaFuncSetAttribute(tma_gemm_ts_kernel<BN, TNR, TNL, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, tsm));
-        NATS_CUDA_OK(cudaFuncSetAttribute(tma_gemm_ts_kernel<BN, TNR, TNL, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, tsm));
-        NATS_CUDA_OK(cudaFuncSetAttribute(tma_gemm_ts_kernel<BN, TNR, TNL, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, tsm));
-        NATS_CUDA_OK(cudaFuncSetAttribute(tma_gemm_ts_kernel<BN, TNR, TNL, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, tsm));
-    }
+template <int BN, bool A_REG>
+int launch_bn(cudaStream_t st, const TmaGroup& grp, bool a_mn, bool b_mn, dim3 grid) {
+    const size_t sm = smem_bytes<BN, A_REG>();
+    cudaError_t e;
+    if (!a_mn && !b_mn) e = launch_pdl(tma_gemm_kernel<BN, false, false, A_REG>, grid, dim3(kThreads), sm, st, grp);
+    else if (!a_mn && b_mn) e = launch_pdl(tma_gemm_kernel<BN, false, true, A_REG>, grid, dim3(kThreads), sm, st, grp);
+    else if (a_mn && !b_mn) e = launch_pdl(tma_gemm_kernel<BN, true, false, A_REG>, grid, dim3(kThreads), sm, st, grp);
+    else e = launch_pdl(tma_gemm_kernel<BN, true, true, A_REG>, grid, dim3(kThreads), sm, st, grp);
+    NATS_CUDA_OK(e);
     return 0;
+}
+
+int g_ts_mode = 1;        // 1: skinny products read the 128-row operand into registers instead of splitting it in shared memory
+
+// operand map: K-major source -> dims (K, rows), box (32, box_rows); MN-major source -> dims (rows, K), box (box_rows, 32)
+int operand_map(const float* ptr, bool mn, int rows, int K, int ld, int batch, long long bstride, int box_rows, CUtensorMap* out) {
+    const long long d0 = mn ? rows : K, d1 = mn ? K : rows;
+    return tma_map_tile3d(ptr, d0, d1, batch, ld, batch > 1 ? bstride : d1 * ld, mn ? box_rows : 32, mn ? 32 : box_rows, 1, out);
 }
 
 }  // namespace
 
-int tma_map_3d(const float* ptr, long long inner, long long outer, long long ld, long long batch, long long bstride,
-               int box_outer, bool mn_major, CUtensorMap* out) {
-    return get_map(ptr, inner, outer, ld, batch, bstride, box_outer, mn_major, out);
-}
 bool tma_available() { return g_encode != nullptr; }
 
 int tma_map_tile3d(const float* ptr, long long d0, long long d1, long long d2, long long stride1, long long stride2, int b0,
@@ -824,8 +310,6 @@ int tma_map_tile3d(const float* ptr, long long d0, long long d1, long long d2, l
     *out = m;
     return 0;
 }
-void tma_gemm_trace(int on) { g_trace_on = on; g_trace_no = 0; }
-void tma_gemm_debug_mode(int mode) { g_dbg_mode = mode; }
 void tma_gemm_set_ts(int on) { g_ts_mode = on; }
 int tma_gemm_get_ts() { return g_ts_mode; }
 
@@ -838,11 +322,13 @@ int tma_gemm_setup() {
         return 1;
     }
     g_encode = reinterpret_cast<EncodeTiledFn>(fn);
-    NATS_TRY((set_attrs<32, 8, 2>()));
-    NATS_TRY((set_attrs<64, 6, 2>()));
-    NATS_TRY((set_attrs<128, 5, 2>()));
+    NATS_TRY((set_attrs<32, false>()));
+    NATS_TRY((set_attrs<64, false>()));
+    NATS_TRY((set_attrs<32, true>()));
+    NATS_TRY((set_attrs<64, true>()));
     return 0;
 }
+
 
 // can this group be served by TMA?  (16-byte aligned pointers, leading dimensions multiple of 4 floats)
 bool tma_gemm_eligible(const GemmProblem* probs, int count) {
@@ -866,7 +352,8 @@ int tma_gemm_launch(cudaStream_t st, const GemmProblem* probs, int count, bool t
     for (int i = 0; i < count; ++i) { maxM = max(maxM, probs[i].M); maxN = max(maxN, probs[i].N); }
     const bool swapped = maxM < 128 && maxN > maxM;
     const int nb_dim = swapped ? maxM : maxN;
-    const int BN = nb_dim <= 32 ? 32 : (nb_dim <= 64 ? 64 : 128);
+    const int BN = nb_dim <= 32 ? 32 : 64;
+    const bool skinny = nb_dim <= 64;
     // op(A)(m,k): transA ? m contiguous : k contiguous.  op(B)(k,n): transB ? k contiguous : n contiguous.
     const bool opa_mn = transA, opb_mn = !transB;
     const bool a_mn = swapped ? opb_mn : opa_mn;      // the 128-row side operand
@@ -877,12 +364,9 @@ int tma_gemm_launch(cudaStream_t st, const GemmProblem* probs, int count, bool t
         const GemmProblem& q = probs[i];
         NATS_REQUIRE(q.splitk >= 1 && q.batch >= 1 && (q.splitk == 1 || !q.accumulate), "tma gemm split/batch");
         TmaProblem& t = grp.p[i];
-        // maps: K-major operand -> inner = K, outer = rows; MN-major -> inner = rows, outer = K
         CUtensorMap ma, mb;
-        NATS_TRY(get_map(q.A, opa_mn ? q.M : q.K, opa_mn ? q.K : q.M, q.lda, q.batch, q.strideA,
-                         opa_mn ? 32 : (swapped ? BN : 128), opa_mn, &ma));
-        NATS_TRY(get_map(q.B, opb_mn ? q.N : q.K, opb_mn ? q.K : q.N, q.ldb, q.batch, q.strideB,
-                         opb_mn ? 32 : (swapped ? 128 : BN), opb_mn, &mb));
+        NATS_TRY(operand_map(q.A, opa_mn, q.M, q.K, q.lda, q.batch, q.strideA, swapped ? BN : 128, &ma));
+        NATS_TRY(operand_map(q.B, opb_mn, q.N, q.K, q.ldb, q.batch, q.strideB, swapped ? 128 : BN, &mb));
         if (!swapped) {
             grp.mapA[i] = ma; grp.mapB[i] = mb;
             t.Ma = q.M; t.Nb = q.N; t.c_rs = q.ldc; t.c_cs = 1; t.bias_on_a = 0;
@@ -896,7 +380,6 @@ int tma_gemm_launch(cudaStream_t st, const GemmProblem* probs, int count, bool t
         if (q.splitk > 1) t.kchunk = ((cdiv(q.K, q.splitk) + 31) / 32) * 32;
         if (t.kchunk <= 0) t.kchunk = 32;
         t.strideP = q.strideP; t.accumulate = q.accumulate;
-        t.a_static = swapped ? q.b_static : q.a_static;
         grp.zstart[i] = z;
         z += q.batch * q.splitk;
         ga = max(ga, cdiv(t.Ma, 128));
@@ -908,9 +391,10 @@ int tma_gemm_launch(cudaStream_t st, const GemmProblem* probs, int count, bool t
     for (int i = count; i < kMaxGroup; ++i) grp.zstart[i + 1] = z;
     if (ga == 0 || gb == 0 || z == 0) return 0;
     dim3 grid(ga, gb, z);
-    if (BN == 32) return launch_bn<32, 8, 2>(st, grp, a_mn, b_mn, grid, flops, bytes);
-    if (BN == 64) return launch_bn<64, 6, 2>(st, grp, a_mn, b_mn, grid, flops, bytes);
-    return launch_bn<128, 5, 2>(st, grp, a_mn, b_mn, grid, flops, bytes);
+    ProfScope ps(st, skinny ? K_TC_GEMM_SKINNY : K_TC_GEMM, flops, bytes);
+    const bool areg = skinny && g_ts_mode;
+    if (BN == 32) return areg ? launch_bn<32, true>(st, grp, a_mn, b_mn, grid) : launch_bn<32, false>(st, grp, a_mn, b_mn, grid);
+    return areg ? launch_bn<64, true>(st, grp, a_mn, b_mn, grid) : launch_bn<64, false>(st, grp, a_mn, b_mn, grid);
 }
 
 }  // namespace nats

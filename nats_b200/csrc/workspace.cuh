@@ -1,4 +1,4 @@
-// workspace.cuh -- flat parameter layout (packed, B200-native) and workspace carving.  Host-side only.
+// workspace.cuh -- flat parameter layout (packed, H100-native) and workspace carving.  Host-side only.
 #pragma once
 #include "common.cuh"
 #include "gemm.cuh"

@@ -1,5 +1,5 @@
 """
-nats_b200.nats -- host side of the B200 implementation of lukecq1231/nats' hot path.
+nats_b200.nats -- host side of the H100 implementation of lukecq1231/nats' hot path.
 
 Same public surface as the reference's scripts/nats.py so that its drivers (train_nats.py, gen.py) keep working:
 
@@ -11,7 +11,7 @@ f_cost, f_grad_shared, f_update -- nats.py:817, 871, 1320, 1336, 1160, 1170) is 
 libnats_b200.so (include/nats_b200.h), called through ctypes with raw device pointers.  PyTorch is used as the
 container for device memory, streams, CUDA graphs and NCCL only.
 
-There is no CPU fallback: without the CUDA library and a B200 the compiled callables raise NatsB200Error.
+There is no CPU fallback: without the CUDA library and an H100 the compiled callables raise NatsB200Error.
 Pure-host helpers (init_params, prepare_data, load_params, the beam bookkeeping of gen_sample) work anywhere.
 """
 from collections import OrderedDict
@@ -260,7 +260,7 @@ class TParams(OrderedDict):
 
 
 def init_tparams(params, engine=None):
-    """numpy dict -> device store (nats.py:72-77).  Needs a B200; prints 'name shape' like the reference."""
+    """numpy dict -> device store (nats.py:72-77).  Needs an H100; prints 'name shape' like the reference."""
     shapes = OrderedDict((k, numpy.shape(v)) for k, v in params.items())
     dims = _dims_from_shapes(shapes)
     engine = engine or get_engine()
@@ -294,7 +294,7 @@ class Engine(object):
         self.torch = torch
         self.lib = _lib.load()
         if not torch.cuda.is_available():
-            raise NatsB200Error('no CUDA device visible: nats_b200 runs on B200 (sm_100a) only, there is no CPU path')
+            raise NatsB200Error('no CUDA device visible: nats_b200 runs on H100 (sm_90a) only, there is no CPU path')
         if device_index is None:
             device_index = int(os.environ.get('LOCAL_RANK', torch.cuda.current_device()))
         torch.cuda.set_device(device_index)

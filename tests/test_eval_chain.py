@@ -12,7 +12,6 @@ import pytest
 from nats_b200 import build_dictionary, evaluate, parallel
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-ROUGE_PL = '/root/reference/scripts/ROUGE.pl'
 
 
 def test_rouge_matches_the_reference_perl_script_goldens():
@@ -28,20 +27,23 @@ def test_rouge_matches_the_reference_perl_script_goldens():
             assert evaluate.format_report(n, metric, evaluate.rouge_lines(ref, hyp, n, metric)) == out, key
 
 
-@pytest.mark.skipif(not os.path.exists(ROUGE_PL), reason='reference checkout not present (GPU box)')
 def test_rouge_against_live_perl(tmp_path):
+    """tests/golden/rouge_seeded.json holds 30 seeded random (reference, system) pairs and the reports the REFERENCE's
+    ROUGE.pl printed for them (ROUGE-1, -2, -L); the files and the command-line entry point must reproduce them."""
+    case = json.load(open(os.path.join(HERE, 'golden', 'rouge_seeded.json')))
     rng = np.random.RandomState(3)
     vocab = ['t%d' % i for i in range(25)]
     ref = [' '.join(rng.choice(vocab, size=rng.randint(1, 40))) for _ in range(30)]
     hyp = [' '.join(rng.choice(vocab, size=rng.randint(0, 40))) for _ in range(30)]
+    assert (ref, hyp) == (case['ref'], case['sys'])
     rp, hp = tmp_path / 'r.txt', tmp_path / 'h.txt'
     rp.write_text('\n'.join(ref) + '\n'); hp.write_text('\n'.join(hyp) + '\n')
     for n, metric in ((1, 'N'), (2, 'N'), (1, 'L')):
-        out = subprocess.run(['perl', ROUGE_PL, str(n), metric, str(rp), str(hp)], capture_output=True, text=True, check=True).stdout
+        out = case['scores']['%d%s' % (n, metric)]
         assert evaluate.format_report(n, metric, evaluate.rouge_file(n, metric, str(rp), str(hp))) == out
     cli = subprocess.run([sys.executable, '-m', 'nats_b200.evaluate', 'rouge', '1', 'L', str(rp), str(hp)], capture_output=True,
                          text=True, check=True, cwd=os.path.dirname(HERE)).stdout
-    assert cli == subprocess.run(['perl', ROUGE_PL, '1', 'L', str(rp), str(hp)], capture_output=True, text=True).stdout
+    assert cli == case['scores']['1L']
 
 
 def test_replace_unk(tmp_path):

@@ -1,4 +1,4 @@
-"""The library's GEMM engine (FFMA and tcgen05 3xTF32 paths) against numpy float64, through nats_debug_gemm."""
+"""The library's GEMM engine (FFMA and wgmma 3xTF32 paths) against numpy float64, through nats_debug_gemm."""
 import ctypes
 
 import numpy as np
@@ -53,9 +53,8 @@ def _run(path, M, N, K, ta, tb, bias=False, accumulate=False, splitk=1, batch=1,
     return np.abs(got - ref).max() / scale
 
 
-# max |err| / sqrt(K) for N(0,1) operands.  FFMA: fp32 rounding only.  tcgen05 3xTF32: the tensor core truncates the
-# accumulator once per MMA (bias ~ -7e-6*sqrt(K) at K = 12800 with the 4-accumulator scheme); single-pass TF32 would
-# sit at ~5e-4, i.e. an order of magnitude above this bound.
+# max |err| / sqrt(K) for N(0,1) operands.  FFMA: fp32 rounding only.  3xTF32: the dropped lo.lo term and the
+# accumulation on the tensor core; single-pass TF32 would sit at ~5e-4, i.e. an order of magnitude above this bound.
 TOL = {0: 1e-5, 1: 5e-5, 2: 5e-5, 3: 5e-5}
 
 SHAPES = [

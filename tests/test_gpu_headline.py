@@ -1,6 +1,7 @@
 """GPU parity AT THE HEADLINE DIMENSIONS (BASELINE configs 3 and 5: D=1000, W=A=100, V=30000, src_len 400 / 800, beam 10)
-against the float64 oracle: these are the shapes on which the persistent tcgen05 encoder (72 + 72 CTAs, 352-deep K chunks),
-the 3-way split-K decoder products, the 224-column TMA slices of the attention kernels and the top-k over 30 k words run.
+against the float64 oracle: these are the shapes on which the persistent wgmma encoder (64 + 64 CTAs per pass, 189-row
+tiles x 4 K chunks forward, 125-row tiles x 8 K chunks backward), the split-K decoder products, the TMA slices of the
+attention kernels and the top-k over 30 k words run.
 Tolerances as everywhere (fp32 path, 3xTF32 products): per-sample cost rel <= 1e-4, every gradient ||g-g*||/||g*|| <= 1e-3,
 f_next probabilities max abs <= 1e-5, identical beam tokens.  Also: every kernel-selection switch of the library is run
 through the parity tests in a subprocess (the switches are read once, at context creation)."""
@@ -191,12 +192,12 @@ def test_config5_beam_vs_oracle(N, params):
 
 
 SWITCHES = [
-    {'NATS_ENC_TC': '0'},                 # per-step encoder path instead of the persistent tcgen05 kernel
+    {'NATS_ENC_TC': '0'},                 # per-step encoder path instead of the persistent tensor-core kernel
     {'NATS_ENC_TC': '2'},                 # persistent forward + per-step backward
     {'NATS_ENC_TC': '3'},                 # per-step forward + persistent backward
     {'NATS_TC': '0'},                     # exact-fp32 FFMA products everywhere
-    {'NATS_TC': '1'},                     # tcgen05 with software loaders (no TMA)
-    {'NATS_TS': '0'},                     # skinny products from shared memory instead of tensor memory
+    {'NATS_TC': '1'},                     # wgmma with software loaders (no TMA)
+    {'NATS_TS': '0'},                     # skinny products split in shared memory instead of registers
     {'NATS_PDL': '0'},                    # no programmatic dependent launch
     # beam-search kernels: one CTA per row / per (row, slice) and library GEMMs instead of the 8-CTA cluster kernels
     {'NATS_TOPK_SIMPLE': '1', 'NATS_SOFTMAX_SIMPLE': '1', 'NATS_ATT_BCAST': '0', 'NATS_NARROW_PROJ': '0'},

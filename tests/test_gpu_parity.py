@@ -460,7 +460,7 @@ def test_full_size_properties(N):
 
 def test_real_dims_vs_oracle(N):
     """LCSTS-shaped dims (BASELINE config 2: D=500, W=A=100, V=4000, Tx=120, Ty=20) with a reduced batch so that the
-    float64 oracle finishes in seconds: the tcgen05 3xTF32 path through 120 recurrent encoder steps and 20 decoder
+    float64 oracle finishes in seconds: the wgmma 3xTF32 path through 120 recurrent encoder steps and 20 decoder
     steps must stay within the fp32 tolerances (cost 1e-4, gradients 1e-3 per tensor)."""
     opts = dict(dim_word=100, dim=500, dim_att=100, n_words=4000, encoder='gru', decoder='gru_cond')
     np.random.seed(4321)

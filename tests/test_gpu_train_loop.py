@@ -1,4 +1,4 @@
-"""End to end through the reference's driver surface on a B200: train() on a tiny synthetic corpus (validation,
+"""End to end through the reference's driver surface on an H100: train() on a tiny synthetic corpus (validation,
 checkpoint, sampling and reload branches of nats.py:1380-1539), then the gen.py path: load_params -> build_sampler ->
 gen_sample with a beam and all three distraction penalties."""
 import os

@@ -131,14 +131,12 @@ def test_text_iterator_and_checkpoint_layout(tmp_path):
 
 
 def test_toy_corpus_runs_through_the_data_path(tmp_path):
-    """BASELINE config 1 plumbing: build a dictionary like data/build_dictionary.py:9-35 does and iterate the toy
-    corpus when it is available (it lives in the read-only reference tree and is absent on the GPU box)."""
-    base = '/root/reference/data'
-    if not os.path.exists(os.path.join(base, 'toy_train_input.txt')):
-        pytest.skip('reference toy corpus not present')
+    """BASELINE config 1 plumbing: build a dictionary like data/build_dictionary.py:9-35 does and iterate the committed
+    cut of the reference's toy corpus (tests/data/toy: the first 128 training pairs)."""
+    base = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'data', 'toy')
     from collections import OrderedDict
     freqs = OrderedDict()
-    with open(os.path.join(base, 'toy_train_input.txt')) as f:
+    with open(os.path.join(base, 'train_input.txt')) as f:
         for line in f:
             for w in line.strip().split(' '):
                 freqs[w] = freqs.get(w, 0) + 1
@@ -150,12 +148,12 @@ def test_toy_corpus_runs_through_the_data_path(tmp_path):
     dic = tmp_path / 'toy.pkl'
     with open(dic, 'wb') as f:
         pickle.dump(worddict, f, protocol=2)
-    it = TextIterator(os.path.join(base, 'toy_train_input.txt'), os.path.join(base, 'toy_train_output.txt'), str(dic),
+    it = TextIterator(os.path.join(base, 'train_input.txt'), os.path.join(base, 'train_output.txt'), str(dic),
                       batch_size=4, n_words=200)
     sx, sy = next(it)
     x, xm, y, ym = N.prepare_data(sx, sy, maxlen=500, n_words=200)
     assert x.shape[1] == 4 and x.max() < 200 and xm.sum(0).min() >= 2 and y.shape[0] == ym.shape[0]
-    assert sum(len(b[0]) for b in [(sx, sy)] + list(it)) == 200
+    assert sum(len(b[0]) for b in [(sx, sy)] + list(it)) == 128
 
 
 def test_device_array_behaves_like_the_host_array_f_next_used_to_return():
