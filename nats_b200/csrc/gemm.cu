@@ -320,7 +320,7 @@ int gemm_pick_split(const nats_ctx* ctx, int M, int N, int K, int groups) {
     int tiles;
     if (g_use_tc && (M >= 128 || N >= 128) && K >= 32) {
         const int a = M > N ? M : N, b = M > N ? N : M;      // 128-row side / N side of the tensor-core tile
-        const int bn = b <= 32 ? 32 : 64;
+        const int bn = b <= 32 ? 32 : b <= 64 ? 64 : b <= 112 ? 112 : 96;     // tile widths of tma_gemm_launch
         tiles = cdiv(a, 128) * cdiv(b, bn);
     } else {
         const int bm = (M <= 32) ? 32 : 64, bn = (M <= 32) ? 128 : 64;
@@ -361,7 +361,7 @@ int gemm_auto(const nats_ctx* ctx, cudaStream_t st, GemmProblem p, bool transA, 
         const bool swapped = p.M < 128 && p.N > p.M;
         const int nb = swapped ? p.M : p.N, ma = swapped ? p.N : p.M;
         (void)a; (void)b;
-        const int bn = nb <= 32 ? 32 : 64;
+        const int bn = nb <= 32 ? 32 : nb <= 64 ? 64 : nb <= 112 ? 112 : 96;
         tiles = (long long)cdiv(ma, 128) * cdiv(nb, bn) * p.batch;
     } else {
         int bm, bn;
@@ -372,15 +372,16 @@ int gemm_auto(const nats_ctx* ctx, cudaStream_t st, GemmProblem p, bool transA, 
     }
     int splits = 1;
     if (tc && p.batch == 1 && tiles >= ctx->num_sms && p.K >= 4096 && scratch != nullptr) {
-        // deep products whose tile count is not a multiple of the SM count (d[U|Ux] of the encoder at dim 1000: 376 tiles of
-        // K = 12768 on 132 SMs = 3 waves for 2.8 waves of work): pick the split-K factor that minimises waves x (k-blocks per
-        // CTA + fixed cost) + the slab reduction.  The costs are a model in microseconds (a 128x64x32 k-block of 3xTF32 against
-        // a fixed cost per CTA and the slab traffic), not measurements.
+        // deep products whose tile count is not a multiple of the SM count (d[U|Ux] of the encoder at dim 1000: 8 x 32 tiles
+        // of 128 x 96, K = 12768, on 132 SMs): pick the split-K factor that minimises waves x (k-blocks per CTA + fixed cost)
+        // + the slab reduction.  The k-block cost is measured: that product unsplit took 1114 us for 2 waves of 399 k-blocks
+        // on an H100 80GB HBM3 at a 400 W power limit, i.e. 1.4 us per 128 x 96 x 32 k-block of 3xTF32.  The fixed cost per
+        // tile and the slab bandwidth (5 TB/s, L2-resident slabs) are estimates.
         double best = 1e30;
         for (int s2 = 1; s2 <= 4; ++s2) {
             if ((long long)s2 * p.M * p.N > scratch_floats) break;
             const long long waves = (tiles * s2 + ctx->num_sms - 1) / ctx->num_sms;
-            double t = (double)waves * ((double)p.K / s2 / 32.0 * 0.75 + 3.0);
+            double t = (double)waves * ((double)p.K / s2 / 32.0 * 1.4 + 3.0);
             if (s2 > 1) t += (double)(s2 + 1) * p.M * p.N * 4.0 / 5.0e6;
             if (t < best) { best = t; splits = s2; }
         }

@@ -8,6 +8,7 @@
 //   Skinny products (the batch, <= 64, on the N side; NATS_TS=1, the default): the 128-row operand (the weights) is NOT
 //   split into shared memory -- each thread reads its wgmma A fragments straight from the raw stage, splits them in
 //   registers and issues the register-A form, so only the small B operand goes through the split pass.
+//   Wider products (N side > 64) run on tma_gemm_kernel_ws below: warp-specialized, persistent, 128 x 96 / 128 x 112 tiles.
 // Requirements: 16-byte aligned base pointers and leading dimensions that are multiples of 4 floats (TMA strides);
 // anything else is served by the software-loader kernel in tc_gemm.cu.
 #include <cuda.h>
@@ -67,6 +68,7 @@ struct alignas(64) TmaGroup {
     CUtensorMap mapB[kMaxGroup];
     TmaProblem p[kMaxGroup];
     int zstart[kMaxGroup + 1];
+    int istart[kMaxGroup + 1];          // first work item of each problem (tma_gemm_kernel_ws)
     int count;
 };
 
@@ -81,12 +83,12 @@ __device__ __forceinline__ float raw_at(uint32_t raw, int r, int k) {
 }
 
 // raw stage -> {hi, lo} K-major SWIZZLE_128B tiles (16-byte chunk c of row r at chunk c ^ (r & 7)); k >= klim reads as 0
-template <int ROWS, bool MN>
+template <int ROWS, bool MN, int NT = kThreads>
 __device__ __forceinline__ void split_tile(uint32_t raw, uint32_t hi_base, uint32_t lo_base, int klim, int tid) {
     constexpr int kChunks = ROWS * 8;
 #pragma unroll
-    for (int i = 0; i < (kChunks + kThreads - 1) / kThreads; ++i) {
-        const int q = tid + i * kThreads;
+    for (int i = 0; i < (kChunks + NT - 1) / NT; ++i) {
+        const int q = tid + i * NT;
         if (q < kChunks) {
             int r, c;
             float4 v;
@@ -246,6 +248,191 @@ __global__ void __launch_bounds__(kThreads, 1) tma_gemm_kernel(const __grid_cons
                   (add_bias && !P.bias_on_a) ? P.bias : nullptr, P.accumulate != 0);
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// Non-skinny products (N side > 64): warp-specialized, persistent 128 x BN tiles (BN = 112 when the N side fits in one,
+// else 96: 1000 x 3000 takes 8 x 32 = 256 tiles, 1.94 waves of 132).
+//   warp 0 (one lane)  TMA producer: kWsNR raw stages of 32 k x (128 A rows | BN B rows) in flight, in the caller's layout.
+//                      The A box is 128-byte swizzled so that the consumers' fragment reads are (nearly) conflict-free.
+//   warps 1-3          split the raw B stage into K-major SWIZZLE_128B tf32 {hi, lo} tiles, a kWsNS-deep ring.
+//   warpgroups 1, 2    consumers, rows 64 (wg - 1) .. + 63: read their A fragments from the raw stage, split them in
+//                      registers and issue the register-A wgmma (m64nBNk8); one commit group per k-step, one in flight.
+// Stages are handed over by full / empty mbarrier pairs (no CTA barrier in the loop), so the producer and the split warps
+// run ahead into the next tile while the consumers store the current one.  The producer warpgroup gives registers to the
+// consumers (setmaxnreg 64 / 216), which hold the three accumulators of tma_gemm_kernel (3 x BN/2) beside the fragments of
+// two k-steps.  (At BN = 128 the three accumulators do not fit and ptxas serializes the wgmma; one accumulator for both
+// A_hi.B_hi halves loses accuracy at deep K.)  Per element the sums are those of tma_gemm_kernel in the same order, so a
+// product with the same split-K factor gives the same bits.
+constexpr int kWsThreads = 384;
+constexpr int kWsNR = 4, kWsNS = 2;
+template <int BN> __host__ __device__ constexpr uint32_t ws_raw() { return 128 * 128 + BN * 128; }    // raw stage: A 16 KB | B
+template <int BN> constexpr size_t ws_smem() { return (size_t)kWsNR * ws_raw<BN>() + (size_t)kWsNS * 2 * BN * 128 + 1024; }
+
+struct WsItem { int g, batch, split, m0, n0, kbeg, kend, nkb; };
+
+template <int BN>
+__device__ __forceinline__ WsItem ws_item(const TmaGroup& grp, int it) {
+    WsItem w;
+    w.g = (grp.count > 1 && it >= grp.istart[1]) ? 1 : 0;
+    const TmaProblem& P = grp.p[w.g];
+    it -= grp.istart[w.g];
+    const int mt = (P.Ma + 127) >> 7, nt = (P.Nb + BN - 1) / BN;
+    w.m0 = (it % mt) * 128; it /= mt;                    // m fastest: concurrent tiles share the B panels in L2
+    w.n0 = (it % nt) * BN; it /= nt;
+    w.split = it % P.splitk; w.batch = it / P.splitk;
+    w.kbeg = w.split * P.kchunk;
+    w.kend = min(P.K, w.kbeg + P.kchunk);
+    w.nkb = (w.kend > w.kbeg) ? (w.kend - w.kbeg + kBlockK - 1) / kBlockK : 0;
+    return w;
+}
+
+// element (r, k) of the raw A stage: K-major [128 rows][128 B] or MN-major 4 x [32 k][32 rows], 128-byte swizzled
+template <bool MN>
+__device__ __forceinline__ float raw_a_sw(uint32_t raw, int r, int k) {
+    const uint32_t off = MN ? (uint32_t)((r >> 5) * 4096 + k * 128 + ((((r & 31) >> 2) ^ (k & 7)) << 4) + (r & 3) * 4)
+                            : (uint32_t)(r * 128 + (((k >> 2) ^ (r & 7)) << 4) + (k & 3) * 4);
+    float v;
+    asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(raw + off));
+    return v;
+}
+template <int N>
+__device__ __forceinline__ void reg_fence_u(uint32_t (&a)[N]) {
+#pragma unroll
+    for (int i = 0; i < N; ++i) asm volatile("" : "+r"(a[i])::"memory");
+}
+
+template <int BN>
+__device__ __forceinline__ void mma_rs_ws(float (&d)[BN / 2], const uint32_t (&a)[4], uint64_t db) {
+    if constexpr (BN == 96) wgmma_rs_n96(d, a, db);
+    else wgmma_rs_n112(d, a, db);
+}
+
+template <int BN, bool A_MN, bool B_MN>
+__global__ void __launch_bounds__(kWsThreads, 1) tma_gemm_kernel_ws(const __grid_constant__ TmaGroup grp, int items) {
+    constexpr uint32_t kRaw = ws_raw<BN>(), kBHalf = BN * 128, kSplit = 2 * kBHalf;
+    constexpr int R = BN / 2;
+    static_assert(BN == 96 || BN == 112, "BN");
+    extern __shared__ __align__(1024) unsigned char smem[];
+    __shared__ __align__(8) uint64_t full[kWsNR], empty[kWsNR], sfull[kWsNS], sempty[kWsNS];
+    // the warp index as a shuffled (provably warp-uniform) value: role branches on it do not serialize the wgmma inside them
+    const int tid = threadIdx.x, warp = __shfl_sync(0xffffffffu, tid >> 5, 0), lane = tid & 31;
+    const uint32_t smem_base = (smem_u32(smem) + 1023u) & ~1023u;
+    const uint32_t split_base = smem_base + kWsNR * kRaw;
+
+    if (tid == 0) {
+        for (int g = 0; g < grp.count; ++g) {
+            asm volatile("prefetch.tensormap [%0];" ::"l"(&grp.mapA[g]) : "memory");
+            asm volatile("prefetch.tensormap [%0];" ::"l"(&grp.mapB[g]) : "memory");
+        }
+        for (int s = 0; s < kWsNR; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 3 + 8); }   // split warps + consumer warps
+        for (int s = 0; s < kWsNS; ++s) { mbar_init(&sfull[s], 3); mbar_init(&sempty[s], 2); }    // split warps / consumer warpgroups
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+    pdl_trigger();
+    pdl_wait();                          // operands and C may be written by the predecessor
+
+    if (warp < 4) {
+        setmaxnreg_dec<64>();
+        if (warp == 0) {
+            if (lane != 0) return;
+            uint32_t kc = 0;
+            for (int it = blockIdx.x; it < items; it += gridDim.x) {
+                const WsItem w = ws_item<BN>(grp, it);
+                const CUtensorMap* mapA = &grp.mapA[w.g];
+                const CUtensorMap* mapB = &grp.mapB[w.g];
+                for (int kb = 0; kb < w.nkb; ++kb, ++kc) {
+                    const int s = kc % kWsNR;
+                    mbar_wait(&empty[s], ((kc / kWsNR) & 1) ^ 1);
+                    const uint32_t raw = smem_base + (uint32_t)s * kRaw;
+                    const int k0 = w.kbeg + kb * kBlockK;
+                    mbar_expect_tx(&full[s], kRaw);
+                    if (A_MN) {
+#pragma unroll
+                        for (int j = 0; j < 4; ++j) tma_load_3d(raw + 4096u * j, mapA, &full[s], w.m0 + 32 * j, k0, w.batch);
+                    } else {
+                        tma_load_3d(raw, mapA, &full[s], k0, w.m0, w.batch);
+                    }
+                    if (B_MN) tma_load_3d(raw + 128 * 128, mapB, &full[s], w.n0, k0, w.batch);
+                    else tma_load_3d(raw + 128 * 128, mapB, &full[s], k0, w.n0, w.batch);
+                }
+            }
+        } else {
+            const int stid = tid - 32;
+            uint32_t kc = 0;
+            for (int it = blockIdx.x; it < items; it += gridDim.x) {
+                const WsItem w = ws_item<BN>(grp, it);
+                for (int kb = 0; kb < w.nkb; ++kb, ++kc) {
+                    const int s = kc % kWsNR, t = kc % kWsNS;
+                    mbar_wait(&full[s], (kc / kWsNR) & 1);
+                    mbar_wait(&sempty[t], ((kc / kWsNS) & 1) ^ 1);
+                    const uint32_t sp = split_base + (uint32_t)t * kSplit;
+                    split_tile<BN, B_MN, 96>(smem_base + (uint32_t)s * kRaw + 128 * 128, sp, sp + kBHalf,
+                                              w.kend - (w.kbeg + kb * kBlockK), stid);
+                    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> wgmma
+                    __syncwarp();
+                    if (lane == 0) { mbar_arrive(&sfull[t]); mbar_arrive(&empty[s]); }
+                }
+            }
+        }
+        return;
+    }
+
+    setmaxnreg_inc<216>();
+    const int ctid = tid - 128, cw = ctid >> 7;
+    const int r0 = 64 * cw + 16 * (warp & 3) + (lane >> 2);     // A fragment rows r0, r0 + 8
+    const int q = lane & 3;
+    uint32_t kc = 0;
+    for (int it = blockIdx.x; it < items; it += gridDim.x) {
+        const WsItem w = ws_item<BN>(grp, it);
+        const TmaProblem& P = grp.p[w.g];
+        float acc0[R], acc1[R], accx[R];
+#pragma unroll
+        for (int i = 0; i < R; ++i) { acc0[i] = 0.f; acc1[i] = 0.f; accx[i] = 0.f; }
+        uint32_t fa[2][2][4] = {};       // [k-step parity][hi, lo][fragment]: the registers of the MMAs in flight
+        for (int kb = 0; kb < w.nkb; ++kb, ++kc) {
+            const int s = kc % kWsNR, t = kc % kWsNS;
+            mbar_wait(&full[s], (kc / kWsNR) & 1);
+            mbar_wait(&sfull[t], (kc / kWsNS) & 1);
+            const uint32_t raw = smem_base + (uint32_t)s * kRaw;
+            const uint32_t sp = split_base + (uint32_t)t * kSplit;
+            const uint64_t b_hi = desc_sw128(sp), b_lo = desc_sw128(sp + kBHalf);
+#pragma unroll
+            for (int kk = 0; kk < 4; ++kk) {
+                uint32_t (&ah)[4] = fa[kk & 1][0];
+                uint32_t (&al)[4] = fa[kk & 1][1];
+                // k beyond the chunk end only occurs at K itself (chunks are multiples of 32), which TMA fills with zeros
+#pragma unroll
+                for (int f = 0; f < 4; ++f) {
+                    const float x = raw_a_sw<A_MN>(raw, r0 + 8 * (f & 1), 8 * kk + q + 4 * (f >> 1));
+                    const float h = to_tf32(x);
+                    ah[f] = __float_as_uint(h);
+                    al[f] = __float_as_uint(to_tf32(x - h));
+                }
+                if (kk == 3) {           // this warp is done reading raw stage s
+                    __syncwarp();
+                    if (lane == 0) mbar_arrive(&empty[s]);
+                }
+                wgmma_fence();
+                mma_rs_ws<BN>(accx, al, b_hi + 2 * kk);
+                mma_rs_ws<BN>(accx, ah, b_lo + 2 * kk);
+                mma_rs_ws<BN>((kk & 1) ? acc1 : acc0, ah, b_hi + 2 * kk);
+                wgmma_commit();
+                wgmma_wait<1>();         // the previous k-step has retired: its fragment registers may be rewritten
+                reg_fence_u(fa[(kk + 1) & 1][0]); reg_fence_u(fa[(kk + 1) & 1][1]);
+                if (kk == 0 && kb > 0 && (ctid & 127) == 0) mbar_arrive(&sempty[(kc - 1) % kWsNS]);
+            }
+        }
+        wgmma_wait<0>();
+        reg_fence(acc0); reg_fence(acc1); reg_fence(accx);
+        reg_fence_u(fa[0][0]); reg_fence_u(fa[0][1]); reg_fence_u(fa[1][0]); reg_fence_u(fa[1][1]);
+        if (w.nkb > 0 && (ctid & 127) == 0) mbar_arrive(&sempty[(kc - 1) % kWsNS]);
+        const bool add_bias = (P.bias != nullptr) && (w.split == 0);
+        gemm_epilogue(acc0, acc1, accx, P.C + (long long)w.batch * P.sC + (long long)w.split * P.strideP, P.c_rs, P.c_cs, P.Ma,
+                      P.Nb, w.m0 + r0, w.n0 + 2 * q, (add_bias && P.bias_on_a) ? P.bias : nullptr,
+                      (add_bias && !P.bias_on_a) ? P.bias : nullptr, P.accumulate != 0);
+    }
+}
+
 template <int BN, bool A_REG>
 constexpr size_t smem_bytes() {
     return (size_t)kNR * (128 * 128 + BN * 128) + 2 * (size_t)(2 * (A_REG ? 0 : 128 * 128) + 2 * BN * 128) + 1024;
@@ -273,6 +460,7 @@ int launch_bn(cudaStream_t st, const TmaGroup& grp, bool a_mn, bool b_mn, dim3 g
     return 0;
 }
 
+int g_num_sms = 0;
 int g_ts_mode = 1;        // 1: skinny products read the 128-row operand into registers instead of splitting it in shared memory
 
 // operand map: K-major source -> dims (K, rows), box (32, box_rows); MN-major source -> dims (rows, K), box (box_rows, 32)
@@ -285,11 +473,13 @@ int operand_map(const float* ptr, bool mn, int rows, int K, int ld, int batch, l
 
 bool tma_available() { return g_encode != nullptr; }
 
-int tma_map_tile3d(const float* ptr, long long d0, long long d1, long long d2, long long stride1, long long stride2, int b0,
-                   int b1, int b2, CUtensorMap* out) {
+namespace {
+int encode_tile3d(const float* ptr, long long d0, long long d1, long long d2, long long stride1, long long stride2, int b0, int b1,
+                  int b2, bool swizzle128, CUtensorMap* out) {
     NATS_REQUIRE(g_encode != nullptr, "tensor maps not available");
-    // cache key reuses MapKey: (inner=d0, outer=d1, ld=stride1, batch=d2, bstride=stride2, box_outer=b0*65536+b1*256+b2, mn=2)
-    MapKey key{ptr, d0, d1, stride1, d2, stride2, b0 * 65536 + b1 * 256 + b2, 2};
+    // cache key reuses MapKey: (inner=d0, outer=d1, ld=stride1, batch=d2, bstride=stride2, box_outer=b0*65536+b1*256+b2,
+    // mn=2 plain / 3 swizzled)
+    MapKey key{ptr, d0, d1, stride1, d2, stride2, b0 * 65536 + b1 * 256 + b2, swizzle128 ? 3 : 2};
     auto it = g_maps.find(key);
     if (it != g_maps.end()) { *out = it->second; return 0; }
     if (g_maps.size() > (1u << 16)) g_maps.clear();
@@ -299,8 +489,8 @@ int tma_map_tile3d(const float* ptr, long long d0, long long d1, long long d2, l
     cuuint32_t estr[3] = {1, 1, 1};
     CUtensorMap m;
     const CUresult r = g_encode(&m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(ptr), gdim, gstr, box, estr,
-                                CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                                CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+                                CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE,
+                                CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) {
         set_error("cuTensorMapEncodeTiled (tile3d) failed (%d): ptr=%p dims=%lld,%lld,%lld strides=%lld,%lld box=%d,%d,%d", (int)r, ptr, d0,
                   d1, d2, stride1, stride2, b0, b1, b2);
@@ -309,6 +499,43 @@ int tma_map_tile3d(const float* ptr, long long d0, long long d1, long long d2, l
     g_maps.emplace(key, m);
     *out = m;
     return 0;
+}
+
+// 128-row side of tma_gemm_kernel_ws, 128-byte swizzled: K-major source -> box (32 k, 128 rows); MN-major source -> box
+// (32 rows, 32 k), four boxes per stage
+int operand_map_ws_a(const float* ptr, bool mn, int rows, int K, int ld, int batch, long long bstride, CUtensorMap* out) {
+    const long long d0 = mn ? rows : K, d1 = mn ? K : rows;
+    return encode_tile3d(ptr, d0, d1, batch, ld, batch > 1 ? bstride : d1 * ld, 32, mn ? 32 : 128, 1, true, out);
+}
+
+template <int BN>
+int set_attrs_ws() {
+    const int sm = (int)ws_smem<BN>();
+    NATS_CUDA_OK(cudaFuncSetAttribute(tma_gemm_kernel_ws<BN, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, sm));
+    NATS_CUDA_OK(cudaFuncSetAttribute(tma_gemm_kernel_ws<BN, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, sm));
+    NATS_CUDA_OK(cudaFuncSetAttribute(tma_gemm_kernel_ws<BN, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, sm));
+    NATS_CUDA_OK(cudaFuncSetAttribute(tma_gemm_kernel_ws<BN, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, sm));
+    return 0;
+}
+
+template <int BN>
+int launch_ws(cudaStream_t st, const TmaGroup& grp, bool a_mn, bool b_mn, int items) {
+    const dim3 grid(min(items, g_num_sms)), block(kWsThreads);     // persistent: one CTA per SM at most
+    const size_t sm = ws_smem<BN>();
+    cudaError_t e;
+    if (!a_mn && !b_mn) e = launch_pdl(tma_gemm_kernel_ws<BN, false, false>, grid, block, sm, st, grp, items);
+    else if (!a_mn && b_mn) e = launch_pdl(tma_gemm_kernel_ws<BN, false, true>, grid, block, sm, st, grp, items);
+    else if (a_mn && !b_mn) e = launch_pdl(tma_gemm_kernel_ws<BN, true, false>, grid, block, sm, st, grp, items);
+    else e = launch_pdl(tma_gemm_kernel_ws<BN, true, true>, grid, block, sm, st, grp, items);
+    NATS_CUDA_OK(e);
+    return 0;
+}
+
+}  // namespace
+
+int tma_map_tile3d(const float* ptr, long long d0, long long d1, long long d2, long long stride1, long long stride2, int b0,
+                   int b1, int b2, CUtensorMap* out) {
+    return encode_tile3d(ptr, d0, d1, d2, stride1, stride2, b0, b1, b2, false, out);
 }
 void tma_gemm_set_ts(int on) { g_ts_mode = on; }
 int tma_gemm_get_ts() { return g_ts_mode; }
@@ -326,6 +553,11 @@ int tma_gemm_setup() {
     NATS_TRY((set_attrs<64, false>()));
     NATS_TRY((set_attrs<32, true>()));
     NATS_TRY((set_attrs<64, true>()));
+    NATS_TRY(set_attrs_ws<96>());
+    NATS_TRY(set_attrs_ws<112>());
+    int dev = 0;
+    NATS_CUDA_OK(cudaGetDevice(&dev));
+    NATS_CUDA_OK(cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev));
     return 0;
 }
 
@@ -352,28 +584,30 @@ int tma_gemm_launch(cudaStream_t st, const GemmProblem* probs, int count, bool t
     for (int i = 0; i < count; ++i) { maxM = max(maxM, probs[i].M); maxN = max(maxN, probs[i].N); }
     const bool swapped = maxM < 128 && maxN > maxM;
     const int nb_dim = swapped ? maxM : maxN;
-    const int BN = nb_dim <= 32 ? 32 : 64;
     const bool skinny = nb_dim <= 64;
+    const int BN = nb_dim <= 32 ? 32 : nb_dim <= 64 ? 64 : nb_dim <= 112 ? 112 : 96;
     // op(A)(m,k): transA ? m contiguous : k contiguous.  op(B)(k,n): transB ? k contiguous : n contiguous.
     const bool opa_mn = transA, opb_mn = !transB;
     const bool a_mn = swapped ? opb_mn : opa_mn;      // the 128-row side operand
     const bool b_mn = swapped ? opa_mn : opb_mn;
-    int z = 0, ga = 0, gb = 0;
+    int z = 0, ga = 0, gb = 0, items = 0;
     double flops = 0.0, bytes = 0.0;
     for (int i = 0; i < count; ++i) {
         const GemmProblem& q = probs[i];
         NATS_REQUIRE(q.splitk >= 1 && q.batch >= 1 && (q.splitk == 1 || !q.accumulate), "tma gemm split/batch");
         TmaProblem& t = grp.p[i];
-        CUtensorMap ma, mb;
-        NATS_TRY(operand_map(q.A, opa_mn, q.M, q.K, q.lda, q.batch, q.strideA, swapped ? BN : 128, &ma));
-        NATS_TRY(operand_map(q.B, opb_mn, q.N, q.K, q.ldb, q.batch, q.strideB, swapped ? 128 : BN, &mb));
-        if (!swapped) {
-            grp.mapA[i] = ma; grp.mapB[i] = mb;
-            t.Ma = q.M; t.Nb = q.N; t.c_rs = q.ldc; t.c_cs = 1; t.bias_on_a = 0;
-        } else {
-            grp.mapA[i] = mb; grp.mapB[i] = ma;
-            t.Ma = q.N; t.Nb = q.M; t.c_rs = 1; t.c_cs = q.ldc; t.bias_on_a = 1;
-        }
+        // the 128-row side (a) and the BN side (b) of the tile
+        const float* pa = swapped ? q.B : q.A;
+        const float* pb = swapped ? q.A : q.B;
+        const int rows_a = swapped ? q.N : q.M, rows_b = swapped ? q.M : q.N;
+        const int ld_a = swapped ? q.ldb : q.lda, ld_b = swapped ? q.lda : q.ldb;
+        const long long s_a = swapped ? q.strideB : q.strideA, s_b = swapped ? q.strideA : q.strideB;
+        if (skinny) NATS_TRY(operand_map(pa, a_mn, rows_a, q.K, ld_a, q.batch, s_a, 128, &grp.mapA[i]));
+        else NATS_TRY(operand_map_ws_a(pa, a_mn, rows_a, q.K, ld_a, q.batch, s_a, &grp.mapA[i]));
+        NATS_TRY(operand_map(pb, b_mn, rows_b, q.K, ld_b, q.batch, s_b, BN, &grp.mapB[i]));
+        t.Ma = rows_a; t.Nb = rows_b;
+        if (!swapped) { t.c_rs = q.ldc; t.c_cs = 1; t.bias_on_a = 0; }
+        else { t.c_rs = 1; t.c_cs = q.ldc; t.bias_on_a = 1; }
         t.C = q.C; t.bias = q.bias; t.K = q.K; t.batch = q.batch; t.sC = q.strideC;
         t.splitk = q.splitk;
         t.kchunk = ((q.kchunk + 31) / 32) * 32;
@@ -381,18 +615,23 @@ int tma_gemm_launch(cudaStream_t st, const GemmProblem* probs, int count, bool t
         if (t.kchunk <= 0) t.kchunk = 32;
         t.strideP = q.strideP; t.accumulate = q.accumulate;
         grp.zstart[i] = z;
+        grp.istart[i] = items;
         z += q.batch * q.splitk;
+        items += q.batch * q.splitk * cdiv(t.Ma, 128) * cdiv(t.Nb, BN);
         ga = max(ga, cdiv(t.Ma, 128));
         gb = max(gb, cdiv(t.Nb, BN));
         flops += 2.0 * q.M * q.N * q.K * q.batch;
         bytes += 4.0 * q.batch * ((double)q.M * q.K + (double)q.K * q.N + (double)q.M * q.N * q.splitk);
     }
     grp.zstart[count] = z;
-    for (int i = count; i < kMaxGroup; ++i) grp.zstart[i + 1] = z;
-    if (ga == 0 || gb == 0 || z == 0) return 0;
-    dim3 grid(ga, gb, z);
+    grp.istart[count] = items;
+    for (int i = count; i < kMaxGroup; ++i) { grp.zstart[i + 1] = z; grp.istart[i + 1] = items; }
+    if (items == 0) return 0;
     ProfScope ps(st, skinny ? K_TC_GEMM_SKINNY : K_TC_GEMM, flops, bytes);
-    const bool areg = skinny && g_ts_mode;
+    if (BN == 112) return launch_ws<112>(st, grp, a_mn, b_mn, items);
+    if (BN == 96) return launch_ws<96>(st, grp, a_mn, b_mn, items);
+    dim3 grid(ga, gb, z);
+    const bool areg = g_ts_mode != 0;
     if (BN == 32) return areg ? launch_bn<32, true>(st, grp, a_mn, b_mn, grid) : launch_bn<32, false>(st, grp, a_mn, b_mn, grid);
     return areg ? launch_bn<64, true>(st, grp, a_mn, b_mn, grid) : launch_bn<64, false>(st, grp, a_mn, b_mn, grid);
 }
