@@ -201,14 +201,14 @@ int nats_beam_reorder_append(nats_ctx_t* ctx, void* stream, const float* src, fl
  *   nats_beam_select : candidate costs hyp_score - log p (nats.py:976), re-ranking with the penalties pen [3,k] or NULL
  *     (:997-999, stored cost un-penalised :1004), the k - dead_k best in flattened-argsort order, then in rank order:
  *     word 0 retires the hypothesis into out_tokens / out_len / out_score (:1037-1041), any other word makes the next
- *     live row.  counters (device int32[8]) = {live_k, dead_k, done, finished, last effective step, -, -, -}; scores [2,k] and tokens [2,k,maxlen] are
+ *     live row.  counters (device int32[8]) = {live_k, dead_k, done, finished, last effective step, sentences done (0 or 1), -, -}; scores [2,k] and tokens [2,k,maxlen] are
  *     ping-pong buffers indexed by step parity; parents [k] (-1 = row unused), next_w [k] (input y of the next step),
  *     fin_parent [k] (parents of the hypotheses retired in this step, compacted, -1 padded) are outputs.
  *   nats_beam_advance: state / acc_ctx / acc_alpha rows of the next step <- outputs of nats_sampler_next gathered by
  *     parents (:1015-1023); histories (alpha always, ctx / state when hist_ctx_src != NULL) <- history of the parent + the
  *     current vectors; out_alpha [k,len_cap,Tx] receives the attention history of the hypotheses retired in this step.
  *     host_counters (NULL = off): page-locked HOST memory the device can address (cudaHostAlloc under unified addressing),
- *     int32[8]; the kernel stores the five counters there as well, so the host polls `done` without any copy.
+ *     int32[8]; the kernel stores the six counters there as well, so the host polls `done` without any copy.
  * The host reads `done` one or two steps late to stop early and copies the result buffers once at the end. */
 int nats_beam_select(nats_ctx_t* ctx, void* stream, const float* top_p, const int32_t* top_i, const float* pen,
                      int k, int maxlen, int step, int32_t* counters, float* scores, int32_t* tokens, int32_t* parents,
@@ -251,6 +251,36 @@ typedef struct nats_beam_step {
     float* hist_alpha_out; float* hist_ctx_out; float* hist_state_out;
 } nats_beam_step_t;
 int nats_beam_step(nats_ctx_t* ctx, void* stream, const nats_dims_t* dims, const nats_beam_step_t* a, int step);
+
+/* One beam step for a GROUP of S source sentences with k rows each, in one call: the weights are read once for all S*k
+ * rows and one chain of kernels runs instead of S.  Every sentence is searched exactly as by nats_beam_step on its own
+ * (the sentences only share launches), and all of them step in lockstep.  nats_beam_step is the S = 1 case with the
+ * source layout [Tx, C].  Row r = s*k + j is row j of sentence s; `beam` holds the fields of nats_beam_step_t with these
+ * layouts (n = S*k):
+ *   ctx [Tx, S, 2*dim], pctx [Tx, S, dim_att]: exactly what nats_sampler_init with x_mask writes for the S sentences
+ *     (Tx = the longest source); src_len [S] (device int32): valid positions of each source.  Attention weights at
+ *     t >= src_len[s] are exactly 0 (the training graph's x_mask, nats.py:538-540), which equals f_next on the unpadded
+ *     source.  alphaT / acc_alpha / the attention histories are Tx wide, with zeros past src_len[s];
+ *   ws: nats_sampler_workspace_bytes(dims, Tx, n);
+ *   next_w [n]; state_* [n, dim]; probs [n, n_words]; alphaT, acc_alpha_* [n, Tx]; ctxs, acc_ctx_* [n, 2*dim];
+ *   hist_alpha_* [n, maxlen, Tx], hist_ctx_* [n, maxlen, 2*dim], hist_state_* [n, maxlen, dim]; scratch >= 3*n*maxlen
+ *     floats, pen [3, n]; top_p / top_i [n, k];
+ *   counters [S, 8] (sentence s: {live_k, dead_k, done, finished, last effective step, -, -, -}; the caller sets every
+ *     sentence to {1, 0, 0, 0, -1, 0, 0, 0}); counters[5] of sentence 0 = number of sentences that are done, counters[6]
+ *     of sentence 0 is used by the kernel and must start at 0;
+ *   scores [2, n], tokens [2, n, maxlen], parents [n], fin_parent [n] (parents are row indices within the sentence);
+ *   out_tokens [S, k, maxlen], out_len [S, k], out_score [S, k], out_alpha [S, k, maxlen, Tx]: sentence s's retired
+ *     hypotheses in slots [0, counters[8*s + 3]);
+ *   host_counters (NULL = off): page-locked host memory, int32[8]; [5] receives the number of sentences that are done
+ *     (for S = 1 also words 0..4), so the host polls one flag for the whole group.
+ * A sentence that is done stays untouched while the others go on.  Errors: k < 1 or k > 32, S < 1, NULL src_len or
+ * buffers. */
+typedef struct nats_beam_step_many {
+    nats_beam_step_t beam;               /* Tx = longest source, k = rows per sentence */
+    int32_t n_src;                       /* S */
+    const int32_t* src_len;              /* [S] device */
+} nats_beam_step_many_t;
+int nats_beam_step_many(nats_ctx_t* ctx, void* stream, const nats_dims_t* dims, const nats_beam_step_many_t* a, int step);
 
 /* ---------------------------------------------------------------- diagnostics ------------------- */
 /* The library's internal GEMM engine, exposed for the parity tests: C = op(A).op(B) (+bias) (+C), row-major,

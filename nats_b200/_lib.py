@@ -38,6 +38,11 @@ class BeamStep(Structure):
                                    'out_score', 'out_alpha', 'host_counters', 'state_next', 'acc_ctx_next',
                                    'acc_alpha_next', 'hist_alpha_out', 'hist_ctx_out', 'hist_state_out')])
 
+
+class BeamStepMany(Structure):
+    """nats_beam_step_many_t of include/nats_b200.h: a group of n_src sentences x k rows"""
+    _fields_ = [('beam', BeamStep), ('n_src', c_int32), ('src_len', _P)]
+
 # name -> (restype, argtypes); mirrors include/nats_b200.h one to one (checked by tests/test_abi.py)
 SIGNATURES = {
     'nats_last_error': (c_char_p, []),
@@ -81,6 +86,7 @@ SIGNATURES = {
     'nats_beam_select': (c_int, [c_void_p, _P, _P, _P, _P, c_int, c_int, c_int, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     'nats_beam_advance': (c_int, [c_void_p, _P] + [_P] * 3 + [c_int] * 6 + [_P] * 16),
     'nats_beam_step': (c_int, [c_void_p, _P, POINTER(Dims), POINTER(BeamStep), c_int]),
+    'nats_beam_step_many': (c_int, [c_void_p, _P, POINTER(Dims), POINTER(BeamStepMany), c_int]),
     'nats_debug_gemm': (c_int, [c_void_p, _P, c_int, c_int, c_int, c_int, c_int, c_int, _P, c_int, _P, c_int, _P, c_int,
                                 _P, c_int, c_int, c_int, c_int64, c_int64, c_int64]),
     'nats_profile_enable': (c_int, [c_void_p, c_int]),

@@ -75,7 +75,7 @@ struct ViewDef { const char* name; int64_t off; int rows, cols, ld, ndim; };
 extern "C" {
 
 const char* nats_last_error(void) { return g_err; }
-int nats_version(void) { return 100; }
+int nats_version(void) { return 101; }
 
 int nats_ctx_create(int device, nats_ctx_t** out) {
     NATS_REQUIRE(out != nullptr, "out");
@@ -376,12 +376,18 @@ int nats_sampler_init(nats_ctx_t* ctx, void* stream, const nats_dims_t* dims, co
     return 0;
 }
 
-int nats_sampler_next(nats_ctx_t* ctx, void* stream, const nats_dims_t* dims, const float* params, const int64_t* y,
-                      const float* ctx_in, int64_t ctx_tstride, int64_t ctx_bstride, const float* pctx_in,
-                      int64_t pctx_tstride, int64_t pctx_bstride, const float* state, const float* acc_ctx,
-                      const float* acc_alpha, int Tx, int n, uint64_t rng_seed, uint64_t rng_step, void* ws,
-                      int64_t ws_bytes, float* probs, int64_t* sample, float* state_out, float* alphaT, float* ctxs,
-                      float* acc_ctx_out, float* acc_alpha_out) {
+}  // extern "C"
+
+namespace {
+
+// f_next on n rows; row b attends to source b / rows_per_src of ctx_in / pctx_in (element (t, s, c) at
+// t * tstride + s * bstride + c), of which src_len[s] positions are valid (NULL: all Tx)
+int sampler_next(nats_ctx_t* ctx, void* stream, const nats_dims_t* dims, const float* params, const int64_t* y,
+                 const float* ctx_in, int64_t ctx_tstride, int64_t ctx_bstride, const float* pctx_in,
+                 int64_t pctx_tstride, int64_t pctx_bstride, int rows_per_src, const int32_t* src_len, const float* state,
+                 const float* acc_ctx, const float* acc_alpha, int Tx, int n, uint64_t rng_seed, uint64_t rng_step, void* ws,
+                 int64_t ws_bytes, float* probs, int64_t* sample, float* state_out, float* alphaT, float* ctxs,
+                 float* acc_ctx_out, float* acc_alpha_out) {
     NATS_REQUIRE(ctx && ws && params && y && ctx_in && state && acc_ctx && acc_alpha, "null argument");
     NATS_REQUIRE(probs && state_out && alphaT && ctxs && acc_ctx_out && acc_alpha_out, "null output");
     NATS_TRY(check_dims(dims));
@@ -420,6 +426,7 @@ int nats_sampler_next(nats_ctx_t* ctx, void* stream, const nats_dims_t* dims, co
     s.n = n; s.Tx = Tx;
     s.h_prev = state; s.xproj = w.xproj_y;
     s.ymask = nullptr; s.xmask = nullptr;                       // mask=None, no context mask (nats.py:472-473, 538)
+    s.rows_per_src = rows_per_src; s.src_len = src_len;         // a source's padding gets alpha = 0 (the x_mask of nats.py:538-540)
     s.pctx = pctx; s.pctx_ts = pts; s.pctx_bs = pbs;
     s.cc = ctx_in; s.cc_ts = ctx_tstride; s.cc_bs = ctx_bstride;
     s.acc_alpha_in = acc_alpha; s.acc_ctx_in = acc_ctx;
@@ -456,6 +463,22 @@ int nats_sampler_next(nats_ctx_t* ctx, void* stream, const nats_dims_t* dims, co
     NATS_TRY(gemm_auto(ctx, st, p, false, false, w.gemm_scratch, w.gemm_scratch_floats));
     NATS_TRY(softmax_sample_rows(st, w.logits, n, V, probs, sample, rng_seed, rng_step));
     return 0;
+}
+
+}  // namespace
+
+extern "C" {
+
+int nats_sampler_next(nats_ctx_t* ctx, void* stream, const nats_dims_t* dims, const float* params, const int64_t* y,
+                      const float* ctx_in, int64_t ctx_tstride, int64_t ctx_bstride, const float* pctx_in,
+                      int64_t pctx_tstride, int64_t pctx_bstride, const float* state, const float* acc_ctx,
+                      const float* acc_alpha, int Tx, int n, uint64_t rng_seed, uint64_t rng_step, void* ws,
+                      int64_t ws_bytes, float* probs, int64_t* sample, float* state_out, float* alphaT, float* ctxs,
+                      float* acc_ctx_out, float* acc_alpha_out) {
+    // a zero batch stride: one source shared by all n rows; otherwise one source per row
+    return sampler_next(ctx, stream, dims, params, y, ctx_in, ctx_tstride, ctx_bstride, pctx_in, pctx_tstride, pctx_bstride,
+                        ctx_bstride == 0 ? n : 1, nullptr, state, acc_ctx, acc_alpha, Tx, n, rng_seed, rng_step, ws, ws_bytes,
+                        probs, sample, state_out, alphaT, ctxs, acc_ctx_out, acc_alpha_out);
 }
 
 // ------------------------------------------------------------------------------------------ optimiser
@@ -497,7 +520,7 @@ int nats_beam_distraction_scores(nats_ctx_t* ctx, void* stream, const float* his
     (void)ctx;
     return beam_distraction_scores(reinterpret_cast<cudaStream_t>(stream), hist_alpha, hist_ctx, hist_state, len_cap,
                                    hist_len, live_k, Tx, C, D, cur_alpha, cur_ctx, cur_state, kl_factor, ctx_factor,
-                                   state_factor, scratch, out);
+                                   state_factor, nullptr, 0, scratch, out);
 }
 int nats_beam_topk(nats_ctx_t* ctx, void* stream, const float* probs, int n, int n_words, int k, int mask_unk,
                    float* out_p, int32_t* out_idx) {
@@ -519,7 +542,7 @@ int nats_beam_select(nats_ctx_t* ctx, void* stream, const float* top_p, const in
     (void)ctx;
     NATS_REQUIRE(top_p && top_i && counters && scores && tokens && parents && next_w && out_tokens && out_len && out_score &&
                      fin_parent, "null argument");
-    return beam_select(reinterpret_cast<cudaStream_t>(stream), top_p, top_i, pen, k, maxlen, step, counters, scores, tokens,
+    return beam_select(reinterpret_cast<cudaStream_t>(stream), top_p, top_i, pen, 1, k, maxlen, step, counters, scores, tokens,
                        parents, reinterpret_cast<long long*>(next_w), out_tokens, out_len, out_score, fin_parent, host_counters);
 }
 
@@ -534,35 +557,68 @@ int nats_beam_advance(nats_ctx_t* ctx, void* stream, const int32_t* parents, con
                      acc_alpha_n && cur_alpha && hist_alpha_src && hist_alpha_dst && out_alpha, "null argument");
     NATS_REQUIRE(hist_ctx_src == nullptr || (hist_ctx_dst && hist_state_src && hist_state_dst && cur_ctx && cur_state),
                  "context / state histories come together");
-    return beam_advance(reinterpret_cast<cudaStream_t>(stream), parents, fin_parent, counters, k, len_cap, step, Tx, C, D,
+    return beam_advance(reinterpret_cast<cudaStream_t>(stream), parents, fin_parent, counters, 1, k, len_cap, step, Tx, C, D,
                         state_o, state_n, acc_ctx_o, acc_ctx_n, acc_alpha_o, acc_alpha_n, cur_alpha, cur_ctx, cur_state,
                         hist_alpha_src, hist_alpha_dst, hist_ctx_src, hist_ctx_dst, hist_state_src, hist_state_dst, out_alpha);
 }
 
-int nats_beam_step(nats_ctx_t* ctx, void* stream, const nats_dims_t* dims, const nats_beam_step_t* a, int step) {
+}  // extern "C"
+
+namespace {
+
+// One beam step of a group of n_src sentences x k rows (nats.py:957-1066 for each sentence): f_next on all rows, each
+// attending to its own source (ctx [Tx, n_src, C]; n_src = 1 with src_len NULL is the single-sentence layout [Tx, C]),
+// distraction scores of the live rows, per-row top-k, one selection warp per sentence, one gather launch.
+int beam_step_group(nats_ctx_t* ctx, cudaStream_t st, const nats_dims_t* dims, const nats_beam_step_t* a, int n_src,
+                    const int32_t* src_len, int step) {
     NATS_REQUIRE(ctx && dims && a, "null argument");
-    NATS_REQUIRE(a->k >= 1 && a->maxlen >= 1 && step >= 0 && step < a->maxlen, "beam step shape");
-    const int D = dims->dim, C = 2 * D, A = dims->dim_att, V = dims->n_words, k = a->k, Tx = a->Tx;
-    NATS_TRY(nats_sampler_next(ctx, stream, dims, a->params, a->next_w, a->ctx, C, 0, a->pctx, A, 0, a->state_in, a->acc_ctx_in,
-                               a->acc_alpha_in, Tx, k, 0, 0, a->ws, a->ws_bytes, a->probs, nullptr, a->state_out, a->alphaT,
-                               a->ctxs, a->acc_ctx_out, a->acc_alpha_out));
+    NATS_REQUIRE(a->k >= 1 && a->k <= 32 && a->maxlen >= 1 && step >= 0 && step < a->maxlen, "beam step shape (1 <= k <= 32)");
+    NATS_REQUIRE(n_src >= 1 && (long long)n_src * a->k <= 65535, "beam group size");
+    NATS_TRY(check_dims(dims));
+    const int D = dims->dim, C = 2 * D, A = dims->dim_att, V = dims->n_words, k = a->k, Tx = a->Tx, n = n_src * k;
+    void* stream = reinterpret_cast<void*>(st);
+    const int64_t cbs = n_src == 1 ? 0 : C, pbs = n_src == 1 ? 0 : A;
+    NATS_TRY(sampler_next(ctx, stream, dims, a->params, a->next_w, a->ctx, (int64_t)n_src * C, cbs, a->pctx, (int64_t)n_src * A,
+                          pbs, k, src_len, a->state_in, a->acc_ctx_in, a->acc_alpha_in, Tx, n, 0, 0, a->ws, a->ws_bytes,
+                          a->probs, nullptr, a->state_out, a->alphaT, a->ctxs, a->acc_ctx_out, a->acc_alpha_out));
     const bool distract = a->kl_factor > 0.f || a->ctx_factor > 0.f || a->state_factor > 0.f;
     const bool use_pen = distract && step > 0;
     if (use_pen) {
         NATS_REQUIRE(a->hist_ctx_in && a->hist_state_in && a->scratch && a->pen, "distraction buffers");
-        NATS_TRY(nats_beam_distraction_scores(ctx, stream, a->hist_alpha_in, a->hist_ctx_in, a->hist_state_in, a->maxlen, step, k,
-                                              Tx, C, D, a->alphaT, a->ctxs, a->state_out, a->kl_factor, a->ctx_factor,
-                                              a->state_factor, a->scratch, a->pen));
+        NATS_TRY(beam_distraction_scores(st, a->hist_alpha_in, a->hist_ctx_in, a->hist_state_in, a->maxlen, step, n, Tx, C, D,
+                                         a->alphaT, a->ctxs, a->state_out, a->kl_factor, a->ctx_factor, a->state_factor,
+                                         a->counters, k, a->scratch, a->pen));
     }
-    NATS_TRY(nats_beam_topk(ctx, stream, a->probs, k, V, k, a->use_unk ? 0 : 1, a->top_p, a->top_i));
-    NATS_TRY(nats_beam_select(ctx, stream, a->top_p, a->top_i, use_pen ? a->pen : nullptr, k, a->maxlen, step, a->counters,
-                              a->scores, a->tokens, a->parents, const_cast<int64_t*>(a->next_w), a->out_tokens, a->out_len,
-                              a->out_score, a->fin_parent, a->host_counters));
-    NATS_TRY(nats_beam_advance(ctx, stream, a->parents, a->fin_parent, a->counters, k, a->maxlen, step, Tx, C, D, a->state_out,
-                               a->state_next, a->acc_ctx_out, a->acc_ctx_next, a->acc_alpha_out, a->acc_alpha_next, a->alphaT,
-                               a->ctxs, a->state_out, a->hist_alpha_in, a->hist_alpha_out, distract ? a->hist_ctx_in : nullptr,
-                               a->hist_ctx_out, a->hist_state_in, a->hist_state_out, a->out_alpha));
+    NATS_REQUIRE(a->probs && a->top_p && a->top_i && a->counters && a->scores && a->tokens && a->parents && a->next_w &&
+                     a->out_tokens && a->out_len && a->out_score && a->fin_parent, "null argument");
+    NATS_REQUIRE(a->state_next && a->acc_ctx_next && a->acc_alpha_next && a->hist_alpha_in && a->hist_alpha_out && a->out_alpha,
+                 "null argument");
+    NATS_REQUIRE(!distract || (a->hist_ctx_out && a->hist_state_out), "distraction histories");
+    NATS_TRY(beam_topk(st, a->probs, n, V, k, a->use_unk ? 0 : 1, a->top_p, a->top_i));
+    NATS_TRY(beam_select(st, a->top_p, a->top_i, use_pen ? a->pen : nullptr, n_src, k, a->maxlen, step, a->counters, a->scores,
+                         a->tokens, a->parents, reinterpret_cast<long long*>(const_cast<int64_t*>(a->next_w)), a->out_tokens,
+                         a->out_len, a->out_score, a->fin_parent, a->host_counters));
+    NATS_TRY(beam_advance(st, a->parents, a->fin_parent, a->counters, n_src, k, a->maxlen, step, Tx, C, D, a->state_out,
+                          a->state_next, a->acc_ctx_out, a->acc_ctx_next, a->acc_alpha_out, a->acc_alpha_next, a->alphaT, a->ctxs,
+                          a->state_out, a->hist_alpha_in, a->hist_alpha_out, distract ? a->hist_ctx_in : nullptr,
+                          a->hist_ctx_out, a->hist_state_in, a->hist_state_out, a->out_alpha));
     return 0;
 }
+
+}  // namespace
+
+extern "C" {
+
+int nats_beam_step(nats_ctx_t* ctx, void* stream, const nats_dims_t* dims, const nats_beam_step_t* a, int step) {
+    return beam_step_group(ctx, reinterpret_cast<cudaStream_t>(stream), dims, a, 1, nullptr, step);
+}
+
+int nats_beam_step_many(nats_ctx_t* ctx, void* stream, const nats_dims_t* dims, const nats_beam_step_many_t* a, int step) {
+    NATS_REQUIRE(a != nullptr, "null argument");
+    NATS_REQUIRE(a->n_src >= 1, "n_src >= 1");
+    NATS_REQUIRE(a->src_len != nullptr, "src_len");
+    return beam_step_group(ctx, reinterpret_cast<cudaStream_t>(stream), dims, &a->beam, a->n_src, a->src_len, step);
+}
+
 
 }  // extern "C"

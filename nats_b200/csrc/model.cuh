@@ -28,6 +28,8 @@ struct DecStep {
     const float* xproj;       // [n,3D]
     const float* ymask;       // [n] or NULL
     const float* xmask;       // [Tx,n] or NULL
+    int rows_per_src;         // row b attends to source b / rows_per_src (0 = 1); see AttFwd
+    const int32_t* src_len;   // [sources] or NULL (= Tx)
     const float* pctx; long long pctx_ts, pctx_bs;
     const float* cc; long long cc_ts, cc_bs;
     const float* acc_alpha_in; const float* acc_ctx_in;

@@ -131,6 +131,7 @@ int decoder_step_forward(const nats_ctx* ctx, cudaStream_t st, const nats_dims_t
         a.ps_save = s.ps_save;
         a.acc_alpha_in = s.acc_alpha_in; a.acc_ctx_in = s.acc_ctx_in;
         a.xmask = s.xmask; a.ymask = s.ymask;
+        a.rows_per_src = s.rows_per_src; a.src_len = s.src_len;
         a.D_wei = params + o.D_wei; a.U_att = params + o.U_att; a.c_att = params + o.c_att;
         a.U_con = params + o.U_con; a.W_con = params + o.W_con;
         a.escore = s.escore;

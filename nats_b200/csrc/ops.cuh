@@ -126,6 +126,8 @@ struct AttFwd {
     const float* acc_alpha_in; // [n,Tx]
     const float* acc_ctx_in;   // [n,C]
     const float* xmask;        // [Tx,n] (element t*n+b) or NULL
+    int rows_per_src;          // row b reads source b / rows_per_src (0 = 1; a zero cc batch stride: all rows share one)
+    const int32_t* src_len;    // [sources] valid positions of each source (alpha = 0 at t >= len) or NULL (= Tx)
     const float* ymask;        // [n] step mask m_ or NULL (= ones)
     const float* D_wei; const float* U_att; const float* c_att; const float* U_con; const float* W_con;
     float* escore;             // [n,Tx] scratch
@@ -185,20 +187,21 @@ int rmsprop_update(cudaStream_t st, long long n, float* p, const float* zg, floa
                    const float* rg2);
 
 // ------------------------------------------------------------------ beam search (nats.py:982-995, 1015-1023)
+// counters (NULL = every row): beam_select's [S][8] counters; rows i with i % k >= live_k of sentence i / k are skipped
 int beam_distraction_scores(cudaStream_t st, const float* hist_alpha, const float* hist_ctx, const float* hist_state,
                             int len_cap, int hist_len, int live_k, int Tx, int C, int D, const float* cur_alpha,
                             const float* cur_ctx, const float* cur_state, float kl, float cf, float sf,
-                            float* scratch, float* out);
+                            const int32_t* counters, int k, float* scratch, float* out);
 // per row the K largest probabilities (descending; ties by ascending index); entry 1 counts as 1e-20 when mask_unk
 int beam_topk(cudaStream_t st, const float* probs, int n, int V, int K, int mask_unk, float* out_p, int32_t* out_idx);
 int beam_reorder_append(cudaStream_t st, const float* src, float* dst, const float* cur, const int32_t* parent,
                         int n_new, int len_cap, int hist_len, int dim);
-// device-resident bookkeeping of one beam step (nats.py:976-1066): see ops_beam.cu
-int beam_select(cudaStream_t st, const float* top_p, const int32_t* top_i, const float* pen, int k, int maxlen, int step,
-                int32_t* counters, float* scores, int32_t* tokens, int32_t* parents, long long* next_w,
+// device-resident bookkeeping of one beam step (nats.py:976-1066) for a group of n_src sentences x k rows: see ops_beam.cu
+int beam_select(cudaStream_t st, const float* top_p, const int32_t* top_i, const float* pen, int n_src, int k, int maxlen,
+                int step, int32_t* counters, float* scores, int32_t* tokens, int32_t* parents, long long* next_w,
                 int32_t* out_tokens, int32_t* out_len, float* out_score, int32_t* fin_parent, int32_t* host_counters);
-int beam_advance(cudaStream_t st, const int32_t* parents, const int32_t* fin_parent, const int32_t* counters, int k,
-                 int len_cap, int step, int Tx, int C, int D, const float* state_o, float* state_n, const float* acc_ctx_o,
+int beam_advance(cudaStream_t st, const int32_t* parents, const int32_t* fin_parent, const int32_t* counters, int n_src,
+                 int k, int len_cap, int step, int Tx, int C, int D, const float* state_o, float* state_n, const float* acc_ctx_o,
                  float* acc_ctx_n, const float* acc_alpha_o, float* acc_alpha_n, const float* cur_alpha, const float* cur_ctx,
                  const float* cur_state, const float* hist_alpha_src, float* hist_alpha_dst, const float* hist_ctx_src,
                  float* hist_ctx_dst, const float* hist_state_src, float* hist_state_dst, float* out_alpha);

@@ -67,6 +67,9 @@ __global__ void __launch_bounds__(kAttThreads) att_scores_kernel(const __grid_co
     float* s_dw = sm + a.A;
     float* s_ua = sm + 2 * a.A;
     const int b = blockIdx.y;
+    const int src = b / a.rows_per_src;
+    const int len = a.src_len ? min(a.Tx, (int)a.src_len[src]) : a.Tx;      // energies past the source are never read
+    const float* pctx_s = a.pctx + (long long)src * a.pctx_bstride;
     for (int i = threadIdx.x; i < a.A; i += blockDim.x) {
         const float s = sum_strided(a.ps_part + (long long)b * a.A + i, a.ps_stride, a.ps_nsplit);
         s_ps[i] = s;
@@ -77,7 +80,7 @@ __global__ void __launch_bounds__(kAttThreads) att_scores_kernel(const __grid_co
     __syncthreads();
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const float catt = __ldg(a.c_att);
-    const int t_end = min(a.Tx, (int)(blockIdx.x + 1) * kRowsPerCta);
+    const int t_end = min(len, (int)(blockIdx.x + 1) * kRowsPerCta);
     if (a.A <= 32 * kScoreAk) {
         // all loads of a row are issued before the first tanh (a runtime-length load/tanh/add loop serialises one
         // memory round trip per 32 columns), and the next row's loads are in flight during this row's arithmetic
@@ -86,7 +89,7 @@ __global__ void __launch_bounds__(kAttThreads) att_scores_kernel(const __grid_co
         int t = blockIdx.x * kRowsPerCta + warp;
         auto fetch = [&](int tt, float (&dst)[kScoreAk], float& av) {
             if (tt < t_end) {
-                const float* pr = a.pctx + (long long)tt * a.pctx_tstride + (long long)b * a.pctx_bstride;
+                const float* pr = pctx_s + (long long)tt * a.pctx_tstride;
                 av = a.acc_alpha_in[(long long)b * a.Tx + tt];
 #pragma unroll
                 for (int k = 0; k < kScoreAk; ++k) dst[k] = (lane + 32 * k < a.A) ? __ldg(pr + lane + 32 * k) : 0.f;
@@ -111,7 +114,7 @@ __global__ void __launch_bounds__(kAttThreads) att_scores_kernel(const __grid_co
     }
     for (int t = blockIdx.x * kRowsPerCta + warp; t < t_end; t += kAttThreads / 32) {
         const float accv = a.acc_alpha_in[(long long)b * a.Tx + t];
-        const float* pr = a.pctx + (long long)t * a.pctx_tstride + (long long)b * a.pctx_bstride;
+        const float* pr = pctx_s + (long long)t * a.pctx_tstride;
         float s = 0.f;
         for (int i = lane; i < a.A; i += 32) s += s_ua[i] * tanhf(__ldg(pr + i) + s_ps[i] + accv * s_dw[i]);
         s = warp_sum(s);
@@ -132,16 +135,18 @@ __global__ void __launch_bounds__(kAttThreads) att_context_kernel(const __grid_c
     uint64_t* bars = reinterpret_cast<uint64_t*>(s_tile + (BULK ? kStages * kStageRows * slice_pad : 0));
 
     const int b = blockIdx.y, tid = threadIdx.x;
+    const int src = b / a.rows_per_src;
+    const int Ts = a.src_len ? min(a.Tx, (int)a.src_len[src]) : a.Tx;     // positions of this row's source
     const int c0 = blockIdx.x * slice_len;
     const int len = min(slice_len, a.C - c0);
-    const float* ccb = a.cc + (long long)b * a.cc_bstride + c0;
-    const int nblk = (a.Tx + kStageRows - 1) / kStageRows;
+    const float* ccb = a.cc + (long long)src * a.cc_bstride + c0;
+    const int nblk = (Ts + kStageRows - 1) / kStageRows;
     const unsigned long long keep_pol = l2_keep_policy(a.cc_keep);
 
     auto issue = [&](int blk) {   // executed by warp 0
         const int stage = blk % kStages;
         const int t0 = blk * kStageRows;
-        const int rows = min(kStageRows, a.Tx - t0);
+        const int rows = min(kStageRows, Ts - t0);
         const int lane = tid & 31;
         if (BULK == 2) {
             // the whole stage is ONE TMA instruction: box (slice_pad columns, 1 sample, 16 positions); out-of-range
@@ -152,13 +157,13 @@ __global__ void __launch_bounds__(kAttThreads) att_context_kernel(const __grid_c
                     asm volatile(
                         "cp.async.bulk.tensor.3d.shared::cluster.global.tile.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1, {%3, %4, %5}], [%2], %6;"
                         ::"r"(smem_u32(s_tile + (long long)stage * kStageRows * slice_pad)), "l"(reinterpret_cast<uint64_t>(&cmap)),
-                        "r"(smem_u32(&bars[stage])), "r"(c0), "r"(b), "r"(t0), "l"(keep_pol)
+                        "r"(smem_u32(&bars[stage])), "r"(c0), "r"(src), "r"(t0), "l"(keep_pol)
                         : "memory");
                 } else {
                     asm volatile(
                         "cp.async.bulk.tensor.3d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
                         ::"r"(smem_u32(s_tile + (long long)stage * kStageRows * slice_pad)), "l"(reinterpret_cast<uint64_t>(&cmap)),
-                        "r"(smem_u32(&bars[stage])), "r"(c0), "r"(b), "r"(t0)
+                        "r"(smem_u32(&bars[stage])), "r"(c0), "r"(src), "r"(t0)
                         : "memory");
                 }
             }
@@ -186,9 +191,10 @@ __global__ void __launch_bounds__(kAttThreads) att_context_kernel(const __grid_c
     }
     pdl_wait();
 
-    // masked softmax over the source positions (nats.py:537-540); max taken over valid positions only
+    // masked softmax over the source positions (nats.py:537-540); max taken over valid positions only; positions past
+    // the row's source get weight 0 exactly
     float lmax = -INFINITY;
-    for (int t = tid; t < a.Tx; t += kAttThreads) {
+    for (int t = tid; t < Ts; t += kAttThreads) {
         const float e = a.escore[(long long)b * a.Tx + t];
         s_alpha[t] = e;
         const float mk = a.xmask ? a.xmask[(long long)t * a.n + b] : 1.f;
@@ -198,6 +204,7 @@ __global__ void __launch_bounds__(kAttThreads) att_context_kernel(const __grid_c
     if (mx == -INFINITY) mx = 0.f;
     float lsum = 0.f;
     for (int t = tid; t < a.Tx; t += kAttThreads) {
+        if (t >= Ts) { s_alpha[t] = 0.f; continue; }
         const float mk = a.xmask ? a.xmask[(long long)t * a.n + b] : 1.f;
         const float w = expf(s_alpha[t] - mx) * mk;
         s_alpha[t] = w;
@@ -214,7 +221,7 @@ __global__ void __launch_bounds__(kAttThreads) att_context_kernel(const __grid_c
             const int stage = blk % kStages;
             mbar_wait(&bars[stage], (uint32_t)((blk / kStages) & 1));
             const int t0 = blk * kStageRows;
-            const int rows = min(kStageRows, a.Tx - t0);
+            const int rows = min(kStageRows, Ts - t0);
             if (tid < len) {
                 const float* tp = s_tile + (long long)stage * kStageRows * slice_pad + tid;
 #pragma unroll 4
@@ -227,14 +234,14 @@ __global__ void __launch_bounds__(kAttThreads) att_context_kernel(const __grid_c
         if (tid < len) {
             const float* p = ccb + tid;
             int t = 0;
-            for (; t + 8 <= a.Tx; t += 8) {
+            for (const int t8 = Ts & ~7; t < t8; t += 8) {
                 float v[8];
 #pragma unroll
                 for (int k = 0; k < 8; ++k) v[k] = __ldg(p + (long long)(t + k) * a.cc_tstride);
 #pragma unroll
                 for (int k = 0; k < 8; ++k) acc = fmaf(s_alpha[t + k], v[k], acc);
             }
-            for (; t < a.Tx; ++t) acc = fmaf(s_alpha[t], __ldg(p + (long long)t * a.cc_tstride), acc);
+            for (; t < Ts; ++t) acc = fmaf(s_alpha[t], __ldg(p + (long long)t * a.cc_tstride), acc);
         }
     }
 
@@ -266,6 +273,8 @@ __global__ void __launch_bounds__(kAttThreads) att_context_kernel(const __grid_c
 // active lanes; here a cluster of 8 CTAs splits the source positions, every CTA walks its positions once for a 128-column
 // group and ALL rows (n <= 16 accumulator sets in registers), the 8 partial sums meet in distributed shared memory in a
 // fixed order, and rank r finishes 16 of the 128 columns (nats.py:541-546, 569-570).
+// Beam search over a group of sentences (rows_per_src = k, src_len set): blockIdx.z = source; its cluster takes the k rows
+// of that source, walks only the source's own positions, and writes alpha = 0 past them.
 constexpr int kBcCluster = 8, kBcCols = 128, kBcMaxN = 16, kBcWarps = kAttThreads / 32;
 
 __global__ void __cluster_dims__(kBcCluster, 1, 1) __launch_bounds__(kAttThreads)
@@ -273,43 +282,58 @@ __global__ void __cluster_dims__(kBcCluster, 1, 1) __launch_bounds__(kAttThreads
     namespace cg = cooperative_groups;
     cg::cluster_group cluster = cg::this_cluster();
     extern __shared__ __align__(16) float bc_sm[];
-    float* s_alpha = bc_sm;                                   // [n][chunk] normalised weights of this CTA's positions
-    float* s_part = bc_sm + (((size_t)a.n * chunk + 3) & ~(size_t)3);   // [n][128] this CTA's partial context (16-byte aligned)
+    const int src = blockIdx.z, r0 = src * a.rows_per_src;       // rows [r0, r0 + nr) read this source
+    const int nr = min(a.rows_per_src, a.n - r0);
+    const int Ts = a.src_len ? min(a.Tx, (int)a.src_len[src]) : a.Tx;
+    float* s_alpha = bc_sm;                                   // [nr][chunk] normalised weights of this CTA's positions
+    float* s_part = bc_sm + (((size_t)a.rows_per_src * chunk + 3) & ~(size_t)3);   // [nr][128] partial context (16-byte aligned)
     __shared__ float s_mx[kBcMaxN], s_inv[kBcMaxN];
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int rank = blockIdx.x, c0 = blockIdx.y * kBcCols;
-    const int t0 = rank * chunk, t1 = min(a.Tx, t0 + chunk);
+    const int my_chunk = (Ts + kBcCluster - 1) / kBcCluster;   // <= chunk (the shared-memory stride)
+    const int t0 = rank * my_chunk, t1 = min(Ts, t0 + my_chunk);
+    const float* ccs = a.cc + (long long)src * a.cc_bstride;
     pdl_trigger();
     pdl_wait();
     // masked softmax statistics of every row over ALL positions (nats.py:537-540); max over valid positions only
-    for (int b = warp; b < a.n; b += kBcWarps) {
+    for (int b = warp; b < nr; b += kBcWarps) {
+        const int row = r0 + b;
         float mx = -INFINITY;
-        for (int t = lane; t < a.Tx; t += 32) {
-            const float mk = a.xmask ? a.xmask[(long long)t * a.n + b] : 1.f;
-            if (mk > 0.f) mx = fmaxf(mx, a.escore[(long long)b * a.Tx + t]);
+        for (int t = lane; t < Ts; t += 32) {
+            const float mk = a.xmask ? a.xmask[(long long)t * a.n + row] : 1.f;
+            if (mk > 0.f) mx = fmaxf(mx, a.escore[(long long)row * a.Tx + t]);
         }
         mx = warp_max(mx);
         if (mx == -INFINITY) mx = 0.f;
         float sum = 0.f;
-        for (int t = lane; t < a.Tx; t += 32) {
-            const float mk = a.xmask ? a.xmask[(long long)t * a.n + b] : 1.f;
-            sum += expf(a.escore[(long long)b * a.Tx + t] - mx) * mk;
+        for (int t = lane; t < Ts; t += 32) {
+            const float mk = a.xmask ? a.xmask[(long long)t * a.n + row] : 1.f;
+            sum += expf(a.escore[(long long)row * a.Tx + t] - mx) * mk;
         }
         sum = warp_sum(sum);
         if (lane == 0) { s_mx[b] = mx; s_inv[b] = 1.f / sum; }
     }
-    for (int i = tid; i < a.n * kBcCols; i += kAttThreads) s_part[i] = 0.f;
+    for (int i = tid; i < nr * kBcCols; i += kAttThreads) s_part[i] = 0.f;
     __syncthreads();
-    for (int i = tid; i < a.n * (t1 - t0); i += kAttThreads) {
-        const int b = i / (t1 - t0), tl = i - b * (t1 - t0), t = t0 + tl;
-        const float mk = a.xmask ? a.xmask[(long long)t * a.n + b] : 1.f;
-        const float al = expf(a.escore[(long long)b * a.Tx + t] - s_mx[b]) * mk * s_inv[b];
+    for (int i = tid; i < nr * (t1 - t0); i += kAttThreads) {
+        const int b = i / (t1 - t0), tl = i - b * (t1 - t0), t = t0 + tl, row = r0 + b;
+        const float mk = a.xmask ? a.xmask[(long long)t * a.n + row] : 1.f;
+        const float al = expf(a.escore[(long long)row * a.Tx + t] - s_mx[b]) * mk * s_inv[b];
         s_alpha[b * chunk + tl] = al;
         if (blockIdx.y == 0) {
-            const float m = a.ymask ? a.ymask[b] : 1.f;
-            const long long o = (long long)b * a.Tx + t;
+            const float m = a.ymask ? a.ymask[row] : 1.f;
+            const long long o = (long long)row * a.Tx + t;
             a.alpha_out[o] = al;
             a.acc_alpha_out[o] = a.acc_alpha_in[o] + m * al;                               // nats.py:570
+        }
+    }
+    if (blockIdx.y == 0 && Ts < a.Tx) {                       // positions past the source: alpha = 0
+        const int pad = a.Tx - Ts;
+        for (int i = rank * kAttThreads + tid; i < nr * pad; i += kBcCluster * kAttThreads) {
+            const int b = i / pad;
+            const long long o = (long long)(r0 + b) * a.Tx + Ts + (i - b * pad);
+            a.alpha_out[o] = 0.f;
+            a.acc_alpha_out[o] = a.acc_alpha_in[o];
         }
     }
     __syncthreads();
@@ -320,7 +344,7 @@ __global__ void __cluster_dims__(kBcCluster, 1, 1) __launch_bounds__(kAttThreads
     for (int b = 0; b < kBcMaxN; ++b) acc[b] = make_float4(0.f, 0.f, 0.f, 0.f);
     const int col = c0 + lane * 4;
     if (col < a.C) {
-        const float* base = a.cc + col;
+        const float* base = ccs + col;
         int t = t0 + warp;
         for (; t + 3 * kBcWarps < t1; t += 4 * kBcWarps) {
             float4 v[4];
@@ -332,7 +356,7 @@ __global__ void __cluster_dims__(kBcCluster, 1, 1) __launch_bounds__(kAttThreads
                 const int tl = t + j * kBcWarps - t0;
 #pragma unroll
                 for (int b = 0; b < kBcMaxN; ++b)
-                    if (b < a.n) {
+                    if (b < nr) {
                         const float al = s_alpha[b * chunk + tl];
                         acc[b].x = fmaf(al, v[j].x, acc[b].x); acc[b].y = fmaf(al, v[j].y, acc[b].y);
                         acc[b].z = fmaf(al, v[j].z, acc[b].z); acc[b].w = fmaf(al, v[j].w, acc[b].w);
@@ -344,7 +368,7 @@ __global__ void __cluster_dims__(kBcCluster, 1, 1) __launch_bounds__(kAttThreads
             const int tl = t - t0;
 #pragma unroll
             for (int b = 0; b < kBcMaxN; ++b)
-                if (b < a.n) {
+                if (b < nr) {
                     const float al = s_alpha[b * chunk + tl];
                     acc[b].x = fmaf(al, v.x, acc[b].x); acc[b].y = fmaf(al, v.y, acc[b].y);
                     acc[b].z = fmaf(al, v.z, acc[b].z); acc[b].w = fmaf(al, v.w, acc[b].w);
@@ -355,7 +379,7 @@ __global__ void __cluster_dims__(kBcCluster, 1, 1) __launch_bounds__(kAttThreads
         if (warp == w) {
 #pragma unroll
             for (int b = 0; b < kBcMaxN; ++b)
-                if (b < a.n) {
+                if (b < nr) {
                     float4* p = reinterpret_cast<float4*>(s_part + b * kBcCols + lane * 4);
                     float4 q = *p;
                     q.x += acc[b].x; q.y += acc[b].y; q.z += acc[b].z; q.w += acc[b].w;
@@ -367,14 +391,14 @@ __global__ void __cluster_dims__(kBcCluster, 1, 1) __launch_bounds__(kAttThreads
     cluster.sync();
     // rank r finishes columns [16 r, 16 r + 16) of the group for every row
     constexpr int kPer = kBcCols / kBcCluster;
-    if (tid < a.n * kPer) {
-        const int b = tid / kPer, cl = rank * kPer + (tid - b * kPer), gc = c0 + cl;
+    if (tid < nr * kPer) {
+        const int b = tid / kPer, cl = rank * kPer + (tid - b * kPer), gc = c0 + cl, row = r0 + b;
         if (gc < a.C) {
             float craw = 0.f;
 #pragma unroll
             for (int q = 0; q < kBcCluster; ++q) craw += cluster.map_shared_rank(s_part, q)[b * kBcCols + cl];
-            const float m = a.ymask ? a.ymask[b] : 1.f;
-            const long long o = (long long)b * a.C + gc;
+            const float m = a.ymask ? a.ymask[row] : 1.f;
+            const long long o = (long long)row * a.C + gc;
             const float accc = a.acc_ctx_in[o];
             const float cv = tanhf(__ldg(a.U_con + gc) * craw + __ldg(a.W_con + gc) * accc);   // nats.py:545-546
             if (a.craw_out) a.craw_out[o] = craw;
@@ -608,19 +632,25 @@ int attention_fwd(const nats_ctx* ctx, cudaStream_t st, const AttFwd& a_in) {
     AttFwd a = a_in;
     a.cc_keep = g_cc_keep;
     NATS_REQUIRE(a.Tx >= 1 && a.n >= 1, "attention shape");
+    if (a.cc_bstride == 0) a.rows_per_src = a.n;           // every row reads the one source
+    if (a.rows_per_src < 1) a.rows_per_src = 1;
+    const int nsrc = cdiv(a.n, a.rows_per_src);
     {
         dim3 grid(cdiv(a.Tx, kRowsPerCta), a.n);
-        ProfScope ps(st, K_ATT_SCORES, 0.0, 4.0 * a.Tx * (a.pctx_bstride == 0 ? 1 : a.n) * a.A);
+        ProfScope ps(st, K_ATT_SCORES, 0.0, 4.0 * a.Tx * (a.pctx_bstride == 0 ? 1 : nsrc) * a.A);
         NATS_CUDA_OK(launch_pdl(att_scores_kernel, grid, dim3(kAttThreads), 3 * a.A * sizeof(float), st, a));
     }
+    // the cluster kernel serves rows grouped by source: one shared source, or the k rows of each sentence of a beam group
     static const int no_bcast = [] { const char* e = getenv("NATS_ATT_BCAST"); return e && atoi(e) == 0; }();
-    if (!no_bcast && a.cc_bstride == 0 && a.n <= kBcMaxN && (a.C & 3) == 0 && (a.cc_tstride & 3) == 0 &&
-        (reinterpret_cast<uintptr_t>(a.cc) & 15) == 0) {
+    if (!no_bcast && (a.cc_bstride == 0 || a.src_len != nullptr) && a.rows_per_src <= kBcMaxN && (a.C & 3) == 0 &&
+        (a.cc_tstride & 3) == 0 && (a.cc_bstride & 3) == 0 && (reinterpret_cast<uintptr_t>(a.cc) & 15) == 0) {
         const int chunk = cdiv(a.Tx, kBcCluster);
-        const size_t smem = ((((size_t)a.n * chunk + 3) & ~(size_t)3) + (size_t)a.n * kBcCols) * sizeof(float);
-        if (smem <= (size_t)g_att_dyn_limit) {
-            ProfScope ps(st, K_ATT_CONTEXT, 2.0 * a.Tx * a.n * a.C, 4.0 * ((double)a.Tx * a.C + 3.0 * a.n * a.Tx + 4.0 * a.n * a.C));
-            NATS_CUDA_OK(launch_pdl(att_context_bcast_kernel, dim3(kBcCluster, cdiv(a.C, kBcCols)), dim3(kAttThreads), smem, st, a, chunk));
+        const size_t rows = (size_t)a.rows_per_src;
+        const size_t smem = (((rows * chunk + 3) & ~(size_t)3) + rows * kBcCols) * sizeof(float);
+        if (smem <= (size_t)g_att_dyn_limit && nsrc <= 65535) {
+            ProfScope ps(st, K_ATT_CONTEXT, 2.0 * a.Tx * a.n * a.C, 4.0 * ((double)a.Tx * nsrc * a.C + 3.0 * a.n * a.Tx + 4.0 * a.n * a.C));
+            NATS_CUDA_OK(launch_pdl(att_context_bcast_kernel, dim3(kBcCluster, cdiv(a.C, kBcCols), nsrc), dim3(kAttThreads), smem, st,
+                                    a, chunk));
             return 0;
         }
     }
@@ -642,11 +672,11 @@ int attention_fwd(const nats_ctx* ctx, cudaStream_t st, const AttFwd& a_in) {
     NATS_REQUIRE(smem <= (size_t)g_att_dyn_limit, "source too long for the attention kernel's shared memory");
     dim3 grid(nslices, a.n);
     ProfScope ps(st, K_ATT_CONTEXT, 2.0 * a.Tx * a.n * a.C,
-                 4.0 * ((double)a.Tx * (a.cc_bstride == 0 ? 1 : a.n) * a.C + 3.0 * a.n * a.Tx + 4.0 * a.n * a.C));
+                 4.0 * ((double)a.Tx * (a.cc_bstride == 0 ? 1 : nsrc) * a.C + 3.0 * a.n * a.Tx + 4.0 * a.n * a.C));
     CUtensorMap cmap;
     memset(&cmap, 0, sizeof(cmap));
-    const bool tiled = bulk && tma_available() && a.cc_bstride >= a.C && a.cc_tstride >= (long long)a.n * a.cc_bstride && slice_pad <= 256;
-    if (tiled) NATS_TRY(tma_map_tile3d(a.cc, a.C, a.n, a.Tx, a.cc_bstride, a.cc_tstride, slice_pad, 1, kStageRows, &cmap));
+    const bool tiled = bulk && tma_available() && a.cc_bstride >= a.C && a.cc_tstride >= (long long)nsrc * a.cc_bstride && slice_pad <= 256;
+    if (tiled) NATS_TRY(tma_map_tile3d(a.cc, a.C, nsrc, a.Tx, a.cc_bstride, a.cc_tstride, slice_pad, 1, kStageRows, &cmap));
     if (tiled) NATS_CUDA_OK(launch_pdl(att_context_kernel<2>, grid, dim3(kAttThreads), smem, st, a, slice, slice_pad, cmap));
     else if (bulk) NATS_CUDA_OK(launch_pdl(att_context_kernel<1>, grid, dim3(kAttThreads), smem, st, a, slice, slice_pad, cmap));
     else NATS_CUDA_OK(launch_pdl(att_context_kernel<0>, grid, dim3(kAttThreads), smem, st, a, slice, slice_pad, cmap));

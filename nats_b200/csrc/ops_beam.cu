@@ -8,15 +8,24 @@ namespace nats {
 
 namespace {
 
+// rows of a beam group that are not live in their sentence (counters [S][8] of beam_select; NULL = every row is live)
+__device__ __forceinline__ bool beam_row_idle(const int32_t* counters, int k, int i) {
+    if (counters == nullptr) return false;
+    const int32_t* c = counters + (i / k) * 8;
+    return c[2] != 0 || i - (i / k) * k >= c[0];
+}
+
 // one CTA per (history step s, hypothesis i): KL(alpha_s || alpha_now), cos-dist(ctx_s, ctx_now), cos-dist(h_s, h_now)
 __global__ void __launch_bounds__(256) beam_pair_kernel(const float* __restrict__ hist_alpha,
                                                         const float* __restrict__ hist_ctx,
                                                         const float* __restrict__ hist_state, int len_cap, int hist_len,
                                                         int Tx, int C, int D, const float* __restrict__ cur_alpha,
                                                         const float* __restrict__ cur_ctx,
-                                                        const float* __restrict__ cur_state, float* __restrict__ scratch) {
+                                                        const float* __restrict__ cur_state, const int32_t* __restrict__ counters,
+                                                        int k, float* __restrict__ scratch) {
     __shared__ float red[32];
     const int s = blockIdx.x, i = blockIdx.y, tid = threadIdx.x;
+    if (beam_row_idle(counters, k, i)) return;
     const long long h = (long long)i * len_cap + s;
     float* out = scratch + ((long long)i * hist_len + s) * 3;
     {   // scipy.stats.entropy(pk, qk): both normalised to sum 1, sum pk*log(pk/qk) with 0*log(0) = 0  (nats.py:990)
@@ -53,9 +62,9 @@ __global__ void __launch_bounds__(256) beam_pair_kernel(const float* __restrict_
 }
 
 __global__ void beam_minmax_kernel(const float* __restrict__ scratch, int hist_len, int live_k, float kl, float cf,
-                                   float sf, float* __restrict__ out) {
+                                   float sf, const int32_t* __restrict__ counters, int k, float* __restrict__ out) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= live_k) return;
+    if (i >= live_k || beam_row_idle(counters, k, i)) return;
     float mn = INFINITY, mc = -INFINITY, ms = -INFINITY;
     for (int s = 0; s < hist_len; ++s) {
         const float* v = scratch + ((long long)i * hist_len + s) * 3;
@@ -81,15 +90,16 @@ __global__ void beam_reorder_kernel(const float* __restrict__ src, float* __rest
 
 int beam_distraction_scores(cudaStream_t st, const float* hist_alpha, const float* hist_ctx, const float* hist_state,
                             int len_cap, int hist_len, int live_k, int Tx, int C, int D, const float* cur_alpha,
-                            const float* cur_ctx, const float* cur_state, float kl, float cf, float sf, float* scratch,
-                            float* out) {
+                            const float* cur_ctx, const float* cur_state, float kl, float cf, float sf, const int32_t* counters,
+                            int k, float* scratch, float* out) {
     NATS_REQUIRE(hist_len >= 1 && live_k >= 1 && hist_len <= len_cap, "beam history shape");
+    NATS_REQUIRE(counters == nullptr || k >= 1, "beam group shape");
     dim3 grid(hist_len, live_k);
     ProfScope ps(st, K_BEAM);
     beam_pair_kernel<<<grid, 256, 0, st>>>(hist_alpha, hist_ctx, hist_state, len_cap, hist_len, Tx, C, D, cur_alpha,
-                                           cur_ctx, cur_state, scratch);
+                                           cur_ctx, cur_state, counters, k, scratch);
     NATS_LAUNCH_OK();
-    beam_minmax_kernel<<<cdiv(live_k, 64), 64, 0, st>>>(scratch, hist_len, live_k, kl, cf, sf, out);
+    beam_minmax_kernel<<<cdiv(live_k, 64), 64, 0, st>>>(scratch, hist_len, live_k, kl, cf, sf, counters, k, out);
     NATS_LAUNCH_OK();
     return 0;
 }
@@ -110,15 +120,40 @@ namespace {
 constexpr int kMaxBeam = 32;
 
 // ---------------------------------------------------------------------------------------------------------------
-// Device-resident beam bookkeeping (nats.py:976-1066), ONE warp: candidate costs from the per-row top-k, distraction
-// re-ranking (nats.py:997-999; the stored cost stays un-penalised, :1004), selection of the k - dead_k best in the
-// stable order of a flattened argsort, then the reference's loop over the selected candidates in rank order: a
-// candidate ending in word 0 retires into the result slots (:1037-1041), the others become the live rows of the next step.
-//   counters[0] live_k, [1] dead_k, [2] done flag (set when live_k < 1 or dead_k >= k, :1057), [3] finished so far,
+// Device-resident beam bookkeeping (nats.py:976-1066), ONE warp per sentence of a group of S (grid S; S = 1 is the
+// single-sentence search): candidate costs from the per-row top-k, distraction re-ranking (nats.py:997-999; the stored cost
+// stays un-penalised, :1004), selection of the k - dead_k best in the stable order of a flattened argsort, then the
+// reference's loop over the selected candidates in rank order: a candidate ending in word 0 retires into the result slots
+// (:1037-1041), the others become the live rows of the next step.  Sentence s owns rows [s k, s k + k) of every per-row
+// buffer, counters[8 s .. 8 s + 8) and its result slots; parents / fin_parent hold row indices local to the sentence.
+//   counters[8 s + 0] live_k, [1] dead_k, [2] done flag (set when live_k < 1 or dead_k >= k, :1057), [3] finished so far,
 //   [4] index of the last step that was carried out (steps issued after `done` change nothing)
+//   counters[5] (sentence 0 only): number of sentences of the group that are done; counters[6]: arrival ticket (kept 0)
 //   scores / tokens are ping-pong buffers selected by the step parity; tokens rows hold `step` words on entry
-//   host_counters (optional): device-visible pinned host memory that receives the same five words
+//   host_counters (optional): device-visible pinned host memory that receives counters[5] (S = 1: also words 0..4)
 // ---------------------------------------------------------------------------------------------------------------
+__device__ __forceinline__ void beam_group_count(int32_t* counters, int32_t* host_counters) {
+    // the last sentence warp to arrive counts the sentences that are done (the others' flags are visible after the fence)
+    const int S = gridDim.x;
+    int nd = -1;
+    if (S == 1) {
+        nd = counters[2] != 0 ? 1 : 0;
+    } else {
+        __threadfence();
+        if (atomicAdd(&counters[6], 1) == S - 1) {
+            nd = 0;
+            for (int s = 0; s < S; ++s) nd += (*(volatile int32_t*)&counters[8 * s + 2] != 0) ? 1 : 0;
+            counters[6] = 0;
+        }
+    }
+    if (nd < 0) return;
+    counters[5] = nd;
+    if (host_counters != nullptr) {
+        *(volatile int32_t*)&host_counters[5] = nd;
+        __threadfence_system();
+    }
+}
+
 __global__ void __launch_bounds__(32) beam_select_kernel(const float* __restrict__ top_p, const int32_t* __restrict__ top_i,
                                                          const float* __restrict__ pen, int k, int maxlen, int step,
                                                          int32_t* __restrict__ counters, float* __restrict__ scores,
@@ -132,14 +167,22 @@ __global__ void __launch_bounds__(32) beam_select_kernel(const float* __restrict
     __shared__ int s_sel[kMaxBeam];
     __shared__ int s_slot[kMaxBeam];                                  // destination row of selected candidate r; bit 30: retired
     const int lane = threadIdx.x;
+    const int sent = blockIdx.x, n = gridDim.x * k, r0 = sent * k;   // this sentence's rows [r0, r0 + k) of n
     const int cur = step & 1, nxt = cur ^ 1;
-    const float* sc_in = scores + cur * k;
-    float* sc_out = scores + nxt * k;
-    const int32_t* tk_in = tokens + (long long)cur * k * maxlen;
-    int32_t* tk_out = tokens + (long long)nxt * k * maxlen;
+    int32_t* cnt = counters + 8 * sent;
+    top_p += (long long)r0 * k; top_i += (long long)r0 * k;
+    const float* sc_in = scores + cur * n + r0;
+    float* sc_out = scores + nxt * n + r0;
+    const int32_t* tk_in = tokens + ((long long)cur * n + r0) * maxlen;
+    int32_t* tk_out = tokens + ((long long)nxt * n + r0) * maxlen;
+    parents += r0; fin_parent += r0; next_w += r0;
+    out_tokens += (long long)r0 * maxlen; out_len += r0; out_score += r0;
     for (int j = lane; j < k; j += 32) { parents[j] = -1; fin_parent[j] = -1; }
-    const int live_k = counters[0], dead_k = counters[1];
-    if (counters[2] != 0) return;                                     // finished earlier: nothing moves any more
+    const int live_k = cnt[0], dead_k = cnt[1];
+    if (cnt[2] != 0) {                                                // finished earlier: nothing moves any more
+        if (lane == 0) beam_group_count(counters, host_counters);
+        return;
+    }
     const int n_keep = k - dead_k;
     const int ncand = live_k * k;
     for (int e = lane; e < k * k; e += 32) {
@@ -151,7 +194,7 @@ __global__ void __launch_bounds__(32) beam_select_kernel(const float* __restrict
             if (word >= 0) {
                 cost = sc_in[r] - logf(top_p[e]);                     // nats.py:976
                 rank = cost;
-                if (pen != nullptr && step > 0) rank = cost + pen[r] + pen[k + r] + pen[2 * k + r];     // :997
+                if (pen != nullptr && step > 0) rank = cost + pen[r0 + r] + pen[n + r0 + r] + pen[2 * n + r0 + r];     // :997
             }
         }
         s_cost[e] = cost;
@@ -178,7 +221,7 @@ __global__ void __launch_bounds__(32) beam_select_kernel(const float* __restrict
         nsel = r + 1;
         __syncwarp();
     }
-    int new_live = 0, nfin = counters[3], ndead = dead_k, fin_now = 0;
+    int new_live = 0, nfin = cnt[3], ndead = dead_k, fin_now = 0;
     for (int r = 0; r < nsel; ++r) {                                  // rank order, as the reference's zip loop (:1010-1052)
         const int e = s_sel[r];
         const int ti = e / k, wi = s_word[e];
@@ -208,19 +251,20 @@ __global__ void __launch_bounds__(32) beam_select_kernel(const float* __restrict
     __syncwarp();
     if (lane == 0) {
         const int done = (new_live < 1 || ndead >= k) ? 1 : 0;
-        counters[0] = new_live; counters[1] = ndead; counters[3] = nfin; counters[4] = step;
-        if (done) counters[2] = 1;
-        if (host_counters != nullptr) {                               // mapped pinned host memory: the host polls it, no copy
+        cnt[0] = new_live; cnt[1] = ndead; cnt[3] = nfin; cnt[4] = step;
+        if (done) cnt[2] = 1;
+        if (host_counters != nullptr && gridDim.x == 1) {             // mapped pinned host memory: the host polls it, no copy
             volatile int32_t* h = host_counters;
             h[0] = new_live; h[1] = ndead; h[3] = nfin; h[4] = step; h[2] = done;
-            __threadfence_system();
         }
+        beam_group_count(counters, host_counters);
     }
 }
 
-// One launch for all the copies of a beam step (nats.py:1015-1023, 1040); blockIdx.z selects the job:
+// One launch for all the copies of a beam step (nats.py:1015-1023, 1040); blockIdx.x = row j of the group (sentence j / k,
+// whose parents are local to its block of k rows), blockIdx.z selects the job:
 //   0..2  history of the next step's row j <- history of its parent + the current vector (alpha; ctx and state when kept)
-//   3     attention history of the hypotheses that retired in this step -> result slot (slots are assigned in order)
+//   3     attention history of the hypotheses that retired in this step -> the sentence's result slot (assigned in order)
 //   4     state / acc_ctx / acc_alpha rows of the next step <- f_next outputs of the parents (blockIdx.y = buffer)
 struct BeamAdvance {
     const int32_t* parents; const int32_t* fin_parent; const int32_t* counters;
@@ -232,29 +276,30 @@ struct BeamAdvance {
 
 __global__ void __launch_bounds__(256) beam_advance_kernel(const __grid_constant__ BeamAdvance a) {
     const int j = blockIdx.x, s = blockIdx.y, job = blockIdx.z;
+    const int r0 = j - j % a.k;                                       // first row of j's sentence
     if (job < 4 && s > a.step) return;                                // the grid is at least 3 deep for job 4
     if (job < 3) {
         if (a.hist_src[job] == nullptr) return;
-        const int par = a.parents[j];
-        if (par < 0) return;                                          // row not alive after this step
+        if (a.parents[j] < 0) return;                                 // row not alive after this step
+        const int par = r0 + a.parents[j];
         const int dim = a.dim[job];
         const float* from = (s < a.step) ? a.hist_src[job] + ((long long)par * a.len_cap + s) * dim : a.cur[job] + (long long)par * dim;
         float* to = a.hist_dst[job] + ((long long)j * a.len_cap + s) * dim;
         for (int t = threadIdx.x; t < dim; t += 256) to[t] = from[t];
     } else if (job == 3) {
-        const int par = a.fin_parent[j];
-        if (par < 0) return;
-        int nf_before = a.counters[3];
+        if (a.fin_parent[j] < 0) return;
+        const int par = r0 + a.fin_parent[j];
+        int nf_before = a.counters[8 * (r0 / a.k) + 3];
         for (int q = 0; q < a.k; ++q)                                 // count this step's retirements
-            if (a.fin_parent[q] >= 0) --nf_before;
+            if (a.fin_parent[r0 + q] >= 0) --nf_before;
         const int Tx = a.dim[0];
         const float* from = (s < a.step) ? a.hist_src[0] + ((long long)par * a.len_cap + s) * Tx : a.cur[0] + (long long)par * Tx;
-        float* to = a.out_alpha + ((long long)(nf_before + j) * a.len_cap + s) * Tx;
+        float* to = a.out_alpha + ((long long)(nf_before + j) * a.len_cap + s) * Tx;    // slot r0 + nf_before + (j - r0)
         for (int t = threadIdx.x; t < Tx; t += 256) to[t] = from[t];
     } else {
         if (s >= 3) return;
-        const int par = a.parents[j];
-        if (par < 0) return;
+        if (a.parents[j] < 0) return;
+        const int par = r0 + a.parents[j];
         const int n = a.row_dim[s];
         const float* src = a.row_src[s] + (long long)par * n;
         float* dst = a.row_dst[s] + (long long)j * n;
@@ -264,23 +309,24 @@ __global__ void __launch_bounds__(256) beam_advance_kernel(const __grid_constant
 
 }  // namespace
 
-int beam_select(cudaStream_t st, const float* top_p, const int32_t* top_i, const float* pen, int k, int maxlen, int step,
-                int32_t* counters, float* scores, int32_t* tokens, int32_t* parents, long long* next_w,
+int beam_select(cudaStream_t st, const float* top_p, const int32_t* top_i, const float* pen, int n_src, int k, int maxlen,
+                int step, int32_t* counters, float* scores, int32_t* tokens, int32_t* parents, long long* next_w,
                 int32_t* out_tokens, int32_t* out_len, float* out_score, int32_t* fin_parent, int32_t* host_counters) {
     NATS_REQUIRE(k >= 1 && k <= kMaxBeam && step >= 0 && step < maxlen, "beam_select shape (beam <= 32)");
+    NATS_REQUIRE(n_src >= 1 && n_src <= 65535, "beam group size");
     ProfScope ps(st, K_BEAM);
-    beam_select_kernel<<<1, 32, 0, st>>>(top_p, top_i, pen, k, maxlen, step, counters, scores, tokens, parents, next_w,
+    beam_select_kernel<<<n_src, 32, 0, st>>>(top_p, top_i, pen, k, maxlen, step, counters, scores, tokens, parents, next_w,
                                          out_tokens, out_len, out_score, fin_parent, host_counters);
     NATS_LAUNCH_OK();
     return 0;
 }
 
-int beam_advance(cudaStream_t st, const int32_t* parents, const int32_t* fin_parent, const int32_t* counters, int k,
-                 int len_cap, int step, int Tx, int C, int D, const float* state_o, float* state_n, const float* acc_ctx_o,
+int beam_advance(cudaStream_t st, const int32_t* parents, const int32_t* fin_parent, const int32_t* counters, int n_src,
+                 int k, int len_cap, int step, int Tx, int C, int D, const float* state_o, float* state_n, const float* acc_ctx_o,
                  float* acc_ctx_n, const float* acc_alpha_o, float* acc_alpha_n, const float* cur_alpha, const float* cur_ctx,
                  const float* cur_state, const float* hist_alpha_src, float* hist_alpha_dst, const float* hist_ctx_src,
                  float* hist_ctx_dst, const float* hist_state_src, float* hist_state_dst, float* out_alpha) {
-    NATS_REQUIRE(k >= 1 && step >= 0 && step < len_cap, "beam_advance shape");
+    NATS_REQUIRE(k >= 1 && n_src >= 1 && step >= 0 && step < len_cap, "beam_advance shape");
     ProfScope ps(st, K_BEAM);
     BeamAdvance a;
     memset(&a, 0, sizeof(a));
@@ -293,7 +339,7 @@ int beam_advance(cudaStream_t st, const int32_t* parents, const int32_t* fin_par
     a.row_src[2] = acc_alpha_o; a.row_dst[2] = acc_alpha_n; a.row_dim[2] = Tx;
     a.out_alpha = out_alpha; a.k = k; a.len_cap = len_cap; a.step = step;
     const int gy = step + 1 < 3 ? 3 : step + 1;
-    beam_advance_kernel<<<dim3(k, gy, 5), 256, 0, st>>>(a);
+    beam_advance_kernel<<<dim3(n_src * k, gy, 5), 256, 0, st>>>(a);
     NATS_LAUNCH_OK();
     return 0;
 }

@@ -921,6 +921,26 @@ def build_sampler(tparams, options, trng=None):
     def _key(x):
         return numpy.ascontiguousarray(x, dtype='int64').reshape(-1).tobytes()
 
+    def encode(vs, slot='init'):
+        """vs: source sentences (1-d word ids) -> init_state [n, D], ctx [Tx, n, C], pctx [Tx, n, A] of ONE masked encoder
+        launch (Tx = the longest; rows t >= len(vs[i]) of column i are padding)"""
+        n = len(vs)
+        Tx = max(len(v) for v in vs)
+        xb = numpy.zeros((Tx, n), dtype='int64')
+        mb = numpy.zeros((Tx, n), dtype='float32')
+        for i, v in enumerate(vs):
+            xb[:len(v), i] = v
+            mb[:len(v), i] = 1.
+        xd, md = torch.from_numpy(xb).to(eng.device), torch.from_numpy(mb).to(eng.device)
+        ws, nbytes = ws_for(Tx, n, slot)
+        f32 = dict(dtype=torch.float32, device=eng.device)
+        init_state, ctx, pctx = torch.empty((n, D), **f32), torch.empty((Tx, n, C), **f32), torch.empty((Tx, n, A), **f32)
+        _lib.check(eng.lib.nats_sampler_init(eng.ctx, eng.stream(), ctypes.byref(dims), _ptr(tparams.flat), _ptr(xd), _ptr(md),
+                                             Tx, n, _ptr(ws), nbytes, _ptr(init_state), _ptr(ctx), _ptr(pctx)),
+                   'nats_sampler_init')
+        eng.launches += 1
+        return init_state, ctx, pctx
+
     def prefetch(xs, max_batch=32):
         """xs: iterable of source sentences ([Tx_i] or [Tx_i, 1] word ids, EOS included); encodes those not parked yet"""
         todo = []
@@ -930,21 +950,7 @@ def build_sampler(tparams, options, trng=None):
                 todo.append((k_, numpy.ascontiguousarray(x, dtype='int64').reshape(-1)))
         for lo in range(0, len(todo), max_batch):
             grp = todo[lo:lo + max_batch]
-            n = len(grp)
-            Tx = max(len(v) for _, v in grp)
-            xb = numpy.zeros((Tx, n), dtype='int64')
-            mb = numpy.zeros((Tx, n), dtype='float32')
-            for i, (_, v) in enumerate(grp):
-                xb[:len(v), i] = v
-                mb[:len(v), i] = 1.
-            xd, md = torch.from_numpy(xb).to(eng.device), torch.from_numpy(mb).to(eng.device)
-            ws, nbytes = ws_for(Tx, n, 'init')
-            f32 = dict(dtype=torch.float32, device=eng.device)
-            init_state, ctx, pctx = torch.empty((n, D), **f32), torch.empty((Tx, n, C), **f32), torch.empty((Tx, n, A), **f32)
-            _lib.check(eng.lib.nats_sampler_init(eng.ctx, eng.stream(), ctypes.byref(dims), _ptr(tparams.flat), _ptr(xd), _ptr(md),
-                                                 Tx, n, _ptr(ws), nbytes, _ptr(init_state), _ptr(ctx), _ptr(pctx)),
-                       'nats_sampler_init')
-            eng.launches += 1
+            init_state, ctx, pctx = encode([v for _, v in grp])
             for i, (k_, v) in enumerate(grp):
                 L = len(v)
                 cache[k_] = (init_state[i].clone(), ctx[:L, i].contiguous(), pctx[:L, i].contiguous())
@@ -968,8 +974,20 @@ def build_sampler(tparams, options, trng=None):
         eng.launches += 1
         return init_state.reshape(D), ctx.reshape(Tx, C), pctx.reshape(Tx, A)
 
+    def init_group(xs):
+        """-> (init_state [S, D], ctx [Tx, S, C], pctx [Tx, S, A], source lengths) of a group of S sentences, used in place by
+        the grouped beam search; ONE sentence goes through init_device (a sentence parked by prefetch is used once)"""
+        if len(xs) == 1:
+            s0, c0, p0 = init_device(xs[0])
+            Tx = int(c0.shape[0])
+            return s0.reshape(1, D), c0.reshape(Tx, 1, C), p0.reshape(Tx, 1, A), [Tx]
+        vs = [numpy.ascontiguousarray(x, dtype='int64').reshape(-1) for x in xs]
+        init_state, ctx, pctx = encode(vs, ('init', eng.stream()))     # per stream, like init_device
+        return init_state, ctx, pctx, [len(v) for v in vs]
+
     f_init.prefetch = prefetch
     f_init.device = init_device
+    f_init.group = init_group
 
     def f_next(y, ctx, init_state, acc_ctx, acc_alpha):
         y = numpy.ascontiguousarray(y, dtype='int64')
@@ -1119,90 +1137,107 @@ def _tile_ctx(ctx0, live_k):
 
 class _DeviceBeam(object):
     """Beam search with every piece of bookkeeping on the device (SURVEY 8(f).1, replaces the host loop of
-    nats.py:1001-1066): per step ONE f_next on k rows (rows >= live_k are ignored), the distraction penalties, a per-row
-    top-k, nats_beam_select (candidate merge, re-ranking, EOS retirement) and nats_beam_advance (state / accumulator /
-    history gathers).  The host reads one 4-byte `done` flag per step, one step late (the GPU queue never drains), and
-    copies tokens, scores and attention histories back once at the end.  Returns the reference's three lists.
+    nats.py:1001-1066), for a GROUP of S source sentences at once: per step ONE f_next on S*k rows (row s*k + j is row j of
+    sentence s and attends to its own source; rows >= live_k of a sentence are ignored), the distraction penalties, a
+    per-row top-k, nats_beam_select (one warp per sentence: candidate merge, re-ranking, EOS retirement) and
+    nats_beam_advance (state / accumulator / history gathers within each sentence).  The weights are read once per step for
+    all S*k rows.  The host reads one 4-byte flag per step, the number of sentences that are done, two steps late (the GPU
+    queue never drains), and copies tokens, scores and attention histories back once at the end.  Each sentence gets the
+    reference's three lists, as its own search would return them.
 
-    One search = one object: __init__ allocates and binds everything on `stream`, step() issues one iteration (False once
-    the search is over), result() fetches the hypotheses.  gen_sample runs a single search on the current stream;
-    gen_sample_many keeps several in flight on separate streams (workspace slot = stream)."""
+    One search = one object: __init__ encodes the group (one masked encoder launch; its [Tx, S, C] output is used in place)
+    and allocates and binds everything on `stream`, step() issues one iteration (False once every sentence is over),
+    result() fetches the hypotheses.  gen_sample runs a group of one on the current stream; gen_sample_many keeps several
+    groups in flight on separate streams (workspace slot = stream).
 
-    def __init__(self, f_init, f_next, x, k, maxlen, use_unk, kl_factor, ctx_factor, state_factor, _trace=None, slot=0,
+    Device memory per group, by count, at S = 16, k = 10, maxlen = 100, Tx = 800, dim = 1000: the ping-pong histories
+    2 x S*k x maxlen x (Tx + 3*dim) floats = 0.49 GB (0.10 GB without penalties), out_alpha S*k x maxlen x Tx floats =
+    0.05 GB, and the f_next workspace of S*k rows, whose encoder part (Tx x S*k x 6*dim floats, unused by the search) makes
+    it 3.2 GB."""
+
+    def __init__(self, f_init, f_next, xs, k, maxlen, use_unk, kl_factor, ctx_factor, state_factor, _trace=None, slot=0,
                  stream=None):
         torch = f_next.engine.torch
         self.tstream = stream if stream is not None else torch.cuda.current_stream(f_next.engine.device)
         with torch.cuda.stream(self.tstream):
-            self._setup(f_init, f_next, x, k, maxlen, use_unk, kl_factor, ctx_factor, state_factor, _trace, slot)
+            self._setup(f_init, f_next, xs, k, maxlen, use_unk, kl_factor, ctx_factor, state_factor, _trace, slot)
 
-    def _setup(self, f_init, f_next, x, k, maxlen, use_unk, kl_factor, ctx_factor, state_factor, _trace, slot):
+    def _setup(self, f_init, f_next, xs, k, maxlen, use_unk, kl_factor, ctx_factor, state_factor, _trace, slot):
         eng = f_next.engine
         torch = eng.torch
         lib = eng.lib
         V, W, D, A = f_next.dims
         C = 2 * D
-        x = numpy.asarray(x)
-        if x.ndim == 2 and x.shape[1] != 1:
-            raise ValueError('gen_sample decodes one source sentence at a time (x is [Tx, 1])')
-        init_state, ctx_d, pctx_d = f_init.device(x)                 # device tensors; parked by f_init.prefetch if it ran
+        S = len(xs)
+        if _trace is not None and S != 1:
+            raise ValueError('the step trace covers a group of one sentence')
+        init_state, ctx_d, pctx_d, src_lens = f_init.group(xs)        # device tensors [S, D], [Tx, S, C], [Tx, S, A]
         Tx = int(ctx_d.shape[0])
+        n = S * k
         dev = eng.device
         f32 = dict(dtype=torch.float32, device=dev)
         i32 = dict(dtype=torch.int32, device=dev)
         distract = kl_factor > 0. or ctx_factor > 0. or state_factor > 0.
         # state of the live rows (ping-pong), f_next outputs, histories, results
-        state = [torch.zeros((k, D), **f32) for _ in range(2)]
-        acc_ctx = [torch.zeros((k, C), **f32) for _ in range(2)]
-        acc_alpha = [torch.zeros((k, Tx), **f32) for _ in range(2)]
-        state[0][0].copy_(init_state.reshape(-1)[:D])
-        outs = [torch.empty((k, V), **f32), None, torch.empty((k, D), **f32),
-                torch.empty((k, Tx), **f32), torch.empty((k, C), **f32), torch.empty((k, C), **f32), torch.empty((k, Tx), **f32)]
-        hist_alpha = [torch.zeros((k, maxlen, Tx), **f32) for _ in range(2)]
-        hist_ctx = [torch.zeros((k, maxlen, C), **f32) for _ in range(2)] if distract else [None, None]
-        hist_state = [torch.zeros((k, maxlen, D), **f32) for _ in range(2)] if distract else [None, None]
-        out_alpha = torch.zeros((k, maxlen, Tx), **f32)
+        state = [torch.zeros((n, D), **f32) for _ in range(2)]
+        acc_ctx = [torch.zeros((n, C), **f32) for _ in range(2)]
+        acc_alpha = [torch.zeros((n, Tx), **f32) for _ in range(2)]
+        state[0].view(S, k, D)[:, 0].copy_(init_state.reshape(S, D))
+        outs = [torch.empty((n, V), **f32), None, torch.empty((n, D), **f32),
+                torch.empty((n, Tx), **f32), torch.empty((n, C), **f32), torch.empty((n, C), **f32), torch.empty((n, Tx), **f32)]
+        hist_alpha = [torch.zeros((n, maxlen, Tx), **f32) for _ in range(2)]
+        hist_ctx = [torch.zeros((n, maxlen, C), **f32) for _ in range(2)] if distract else [None, None]
+        hist_state = [torch.zeros((n, maxlen, D), **f32) for _ in range(2)] if distract else [None, None]
+        out_alpha = torch.zeros((S, k, maxlen, Tx), **f32)
         c0 = getattr(eng, '_beam_counters0', None)               # live_k, dead_k, done, finished, last effective step
         if c0 is None:                                           # (a host list -> device tensor is a synchronous copy: once)
             c0 = eng._beam_counters0 = torch.tensor([1, 0, 0, 0, -1, 0, 0, 0], **i32)
-        counters = c0.clone()
-        scores = torch.zeros((2, k), **f32)
-        tokens = torch.zeros((2, k, maxlen), **i32)
-        parents = torch.zeros((k,), **i32)
-        fin_parent = torch.zeros((k,), **i32)
-        next_w = torch.full((k,), -1, dtype=torch.int64, device=dev)          # BOS marker -> zero embedding
-        out_tokens = torch.zeros((k, maxlen), **i32)
-        out_len = torch.zeros((k,), **i32)
-        out_score = torch.zeros((k,), **f32)
-        top_p, top_i = torch.empty((k, k), **f32), torch.empty((k, k), **i32)
-        pen = torch.zeros((3 * k,), **f32)
-        scratch = torch.zeros((3 * k * maxlen + 16,), **f32)
-        # `done` reaches the host without a copy: nats_beam_select mirrors the counters into pinned host memory, the loop looks at
-        # them two steps late (after that step's event), so the GPU queue never drains.  All pointer arguments are converted
-        # once, per ping-pong parity: the loop body is five C calls on prebuilt tuples.
+        counters = c0.repeat(S)
+        src_len_h = torch.tensor(src_lens, dtype=torch.int32).pin_memory()
+        src_len = src_len_h.to(dev, non_blocking=True)
+        scores = torch.zeros((2, n), **f32)
+        tokens = torch.zeros((2, n, maxlen), **i32)
+        parents = torch.zeros((n,), **i32)
+        fin_parent = torch.zeros((n,), **i32)
+        next_w = torch.full((n,), -1, dtype=torch.int64, device=dev)          # BOS marker -> zero embedding
+        out_tokens = torch.zeros((S, k, maxlen), **i32)
+        out_len = torch.zeros((S, k), **i32)
+        out_score = torch.zeros((S, k), **f32)
+        top_p, top_i = torch.empty((n, k), **f32), torch.empty((n, k), **i32)
+        pen = torch.zeros((3 * n,), **f32)
+        scratch = torch.zeros((3 * n * maxlen + 16,), **f32)
+        # the number of sentences that are done reaches the host without a copy: nats_beam_select mirrors it into pinned host
+        # memory, the loop looks at it two steps late (after that step's event), so the GPU queue never drains.  All pointer
+        # arguments are converted once, per ping-pong parity: the loop body is one C call on a prebuilt struct.
         host_cnt = torch.zeros(8, dtype=torch.int32).pin_memory()
         host_np = host_cnt.numpy()
         events = [torch.cuda.Event() for _ in range(2)]
         P, cf = _ptr, ctypes.c_float
         stream = ctypes.c_void_p(self.tstream.cuda_stream)
-        step_next = [f_next.bind_next(next_w, ctx_d, pctx_d, state[c], acc_ctx[c], acc_alpha[c], Tx, k, outs) for c in (0, 1)]
-        pen_head = [(eng.ctx, stream, P(hist_alpha[c]), P(hist_ctx[c]), P(hist_state[c]), maxlen) for c in (0, 1)]
-        pen_tail = (k, Tx, C, D, P(outs[3]), P(outs[4]), P(outs[2]), cf(kl_factor), cf(ctx_factor), cf(state_factor), P(scratch), P(pen))
-        topk_args = (eng.ctx, stream, P(outs[0]), k, V, k, 0 if use_unk else 1, P(top_p), P(top_i))
-        sel_head = (eng.ctx, stream, P(top_p), P(top_i))
-        sel_tail = (P(counters), P(scores), P(tokens), P(parents), P(next_w), P(out_tokens), P(out_len), P(out_score), P(fin_parent),
-                    P(host_cnt))
-        pen_ptr, no_ptr = P(pen), P(None)
-        adv_head = (eng.ctx, stream, P(parents), P(fin_parent), P(counters), k, maxlen)
-        adv_tail = [(Tx, C, D, P(outs[2]), P(state[c ^ 1]), P(outs[5]), P(acc_ctx[c ^ 1]), P(outs[6]), P(acc_alpha[c ^ 1]),
-                     P(outs[3]), P(outs[4]), P(outs[2]), P(hist_alpha[c]), P(hist_alpha[c ^ 1]), P(hist_ctx[c]), P(hist_ctx[c ^ 1]),
-                     P(hist_state[c]), P(hist_state[c ^ 1]), P(out_alpha)) for c in (0, 1)]
+        if _trace is not None:                                   # five separate calls per step (single sentence, [Tx, C])
+            ctx1, pctx1 = ctx_d.reshape(Tx, C), pctx_d.reshape(Tx, A)
+            step_next = [f_next.bind_next(next_w, ctx1, pctx1, state[c], acc_ctx[c], acc_alpha[c], Tx, k, outs) for c in (0, 1)]
+            pen_head = [(eng.ctx, stream, P(hist_alpha[c]), P(hist_ctx[c]), P(hist_state[c]), maxlen) for c in (0, 1)]
+            pen_tail = (k, Tx, C, D, P(outs[3]), P(outs[4]), P(outs[2]), cf(kl_factor), cf(ctx_factor), cf(state_factor), P(scratch),
+                        P(pen))
+            topk_args = (eng.ctx, stream, P(outs[0]), k, V, k, 0 if use_unk else 1, P(top_p), P(top_i))
+            sel_head = (eng.ctx, stream, P(top_p), P(top_i))
+            sel_tail = (P(counters), P(scores), P(tokens), P(parents), P(next_w), P(out_tokens), P(out_len), P(out_score),
+                        P(fin_parent), P(host_cnt))
+            pen_ptr, no_ptr = P(pen), P(None)
+            adv_head = (eng.ctx, stream, P(parents), P(fin_parent), P(counters), k, maxlen)
+            adv_tail = [(Tx, C, D, P(outs[2]), P(state[c ^ 1]), P(outs[5]), P(acc_ctx[c ^ 1]), P(outs[6]), P(acc_alpha[c ^ 1]),
+                         P(outs[3]), P(outs[4]), P(outs[2]), P(hist_alpha[c]), P(hist_alpha[c ^ 1]), P(hist_ctx[c]),
+                         P(hist_ctx[c ^ 1]), P(hist_state[c]), P(hist_state[c ^ 1]), P(out_alpha)) for c in (0, 1)]
         check = _lib.check
-        # without a trace the whole step is ONE foreign call (nats_beam_step) on a prebuilt argument struct per parity
+        # without a trace the whole step is ONE foreign call (nats_beam_step_many) on a prebuilt argument struct per parity
         ws_for, tp_, dims_ = f_next.beam_env
-        ws_t, ws_bytes = ws_for(Tx, k, slot)
+        ws_t, ws_bytes = ws_for(Tx, n, slot)
         one_call = []
         for c in (0, 1):
-            a = _lib.BeamStep()
+            m = _lib.BeamStepMany()
+            m.n_src, m.src_len = S, src_len.data_ptr()
+            a = m.beam
             a.params, a.next_w, a.ctx, a.pctx = tp_.flat.data_ptr(), next_w.data_ptr(), ctx_d.data_ptr(), pctx_d.data_ptr()
             a.Tx, a.k, a.maxlen, a.use_unk = Tx, k, maxlen, 1 if use_unk else 0
             a.ws, a.ws_bytes = ws_t.data_ptr(), ws_bytes
@@ -1221,7 +1256,7 @@ class _DeviceBeam(object):
             a.hist_alpha_out = hist_alpha[c ^ 1].data_ptr()
             a.hist_ctx_out = hist_ctx[c ^ 1].data_ptr() if distract else None
             a.hist_state_out = hist_state[c ^ 1].data_ptr() if distract else None
-            one_call.append((eng.ctx, stream, ctypes.byref(dims_), ctypes.byref(a)))
+            one_call.append((eng.ctx, stream, ctypes.byref(dims_), ctypes.byref(m)))
         # every local becomes an attribute: step() / result() use a dozen of them, and ALL the tensors above must outlive the
         # search because their addresses sit in the prebuilt argument structs (a tensor dropped here would be a dangling pointer)
         keep = dict(locals())
@@ -1230,7 +1265,8 @@ class _DeviceBeam(object):
         self.ii = 0
 
     def step(self):
-        """issue iteration self.ii; False when the search has ended (all hypotheses retired, or maxlen reached)"""
+        """issue iteration self.ii; False when the search has ended (every sentence retired all its hypotheses or
+        maxlen was reached)"""
         ii, maxlen, torch = self.ii, self.maxlen, self.torch
         if ii >= maxlen:
             return False
@@ -1238,15 +1274,15 @@ class _DeviceBeam(object):
         events = self.events
         if ii >= 2:
             events[cur].synchronize()                         # step ii-2 is through: its counters are in host memory
-            if self.host_np[2] != 0:
+            if self.host_np[5] >= self.S:
                 self.ii = maxlen
                 return False
         self.ii = ii + 1
         eng = self.eng
         if self._trace is None:
-            rc = self.lib.nats_beam_step(*self.one_call[cur], ii)
+            rc = self.lib.nats_beam_step_many(*self.one_call[cur], ii)
             if rc != 0:
-                self.check(rc, 'nats_beam_step')
+                self.check(rc, 'nats_beam_step_many')
             eng.launches += 1
             events[cur].record(self.tstream)
             return True
@@ -1267,58 +1303,68 @@ class _DeviceBeam(object):
         return True
 
     def result(self):
-        """the reference's three lists (nats.py:1068-1076): retired hypotheses first, then what is still alive"""
+        """per sentence of the group, the reference's three lists (nats.py:1068-1076): retired hypotheses first, then what
+        is still alive; attention rows are cut to the sentence's own length"""
         torch = self.torch
         with torch.cuda.stream(self.tstream):
             out = self._result()
         return out
 
     def _result(self):
-        counters, out_tokens, out_len, out_score, out_alpha = self.counters, self.out_tokens, self.out_len, self.out_score, self.out_alpha
-        tokens, scores, hist_alpha = self.tokens, self.scores, self.hist_alpha
+        S, k = self.S, self.k
         self.tstream.synchronize()
-        cnt = counters.cpu().numpy()
-        live_k, n_fin = int(cnt[0]), int(cnt[3])
-        # with the late flag up to two steps may have run after `done`: nats_beam_select leaves everything untouched then
-        fin_tok, fin_len, fin_sc = out_tokens.cpu().numpy(), out_len.cpu().numpy(), out_score.cpu().numpy()
-        fin_al = out_alpha.cpu().numpy()
-        sample, sample_score, sample_dec_alphas = [], [], []
-        for f in range(n_fin):
-            L = int(fin_len[f])
-            sample.append([int(t) for t in fin_tok[f, :L]])
-            sample_score.append(numpy.float32(fin_sc[f]))
-            sample_dec_alphas.append(list(fin_al[f, :L].copy()))       # one copy; the rows are views of it
-        if live_k > 0:                                            # dump what is still alive (nats.py:1068-1074)
-            s_last = int(cnt[4])                                  # step s wrote the rows of parity (s + 1) & 1, s + 1 words each
-            par, L = (s_last + 1) & 1, s_last + 1
-            lt, ls, ha = tokens[par].cpu().numpy(), scores[par].cpu().numpy(), hist_alpha[par].cpu().numpy()
-            for j in range(live_k):
-                sample.append([int(t) for t in lt[j, :L]])
-                sample_score.append(numpy.float32(ls[j]))
-                sample_dec_alphas.append(list(ha[j, :L].copy()))
-        return sample, sample_score, sample_dec_alphas
+        cnt = self.counters.cpu().numpy().reshape(S, 8)
+        # with the late flag up to two steps may have run after `done`: nats_beam_select leaves a done sentence untouched
+        fin_tok, fin_len, fin_sc = self.out_tokens.cpu().numpy(), self.out_len.cpu().numpy(), self.out_score.cpu().numpy()
+        fin_al = self.out_alpha.cpu().numpy()
+        live = {}                                             # parity -> host copies of the live rows' buffers
+        res = []
+        for s in range(S):
+            live_k, n_fin, Ls = int(cnt[s, 0]), int(cnt[s, 3]), self.src_lens[s]
+            sample, sample_score, sample_dec_alphas = [], [], []
+            for f in range(n_fin):
+                L = int(fin_len[s, f])
+                sample.append([int(t) for t in fin_tok[s, f, :L]])
+                sample_score.append(numpy.float32(fin_sc[s, f]))
+                sample_dec_alphas.append(list(fin_al[s, f, :L, :Ls].copy()))     # one copy; the rows are views of it
+            if live_k > 0:                                    # dump what is still alive (nats.py:1068-1074)
+                s_last = int(cnt[s, 4])                       # step s_last wrote the rows of parity (s_last + 1) & 1
+                par, L = (s_last + 1) & 1, s_last + 1
+                if par not in live:
+                    live[par] = (self.tokens[par].cpu().numpy(), self.scores[par].cpu().numpy(),
+                                 self.hist_alpha[par].cpu().numpy())
+                lt, ls, ha = live[par]
+                for j in range(s * k, s * k + live_k):
+                    sample.append([int(t) for t in lt[j, :L]])
+                    sample_score.append(numpy.float32(ls[j]))
+                    sample_dec_alphas.append(list(ha[j, :L, :Ls].copy()))
+            res.append((sample, sample_score, sample_dec_alphas))
+        return res
 
 
 def _gen_sample_device(f_init, f_next, x, k, maxlen, use_unk, kl_factor, ctx_factor, state_factor, _trace):
-    """one device-resident beam search on the current stream (see _DeviceBeam)"""
-    b = _DeviceBeam(f_init, f_next, x, k, maxlen, use_unk, kl_factor, ctx_factor, state_factor, _trace)
+    """one device-resident beam search (a group of one sentence) on the current stream (see _DeviceBeam)"""
+    b = _DeviceBeam(f_init, f_next, [x], k, maxlen, use_unk, kl_factor, ctx_factor, state_factor, _trace)
     while b.step():
         pass
-    return b.result()
+    return b.result()[0]
 
 
 def gen_sample_many(tparams, f_init, f_next, xs, options, trng=None, k=5, maxlen=30, use_unk=False, kl_factor=0,
                     ctx_factor=0, state_factor=0, concurrency=12, chunk=16):
     """Beam search (nats.py:879-1076, stochastic=False) of a LIST of source sentences -> list of gen_sample's three lists.
-    A beam step is a chain of ~18 small dependent kernels that leaves most of the GPU idle and costs the host ~40 us to
-    issue against ~180 us of device time, so `concurrency` searches run interleaved, each on its own CUDA stream with its
-    own workspace (measured: 210 / 281 / 332 / 375 / 407 sentences/s with 1 / 2 / 4 / 8 / 12 in flight); the encoders of every `chunk` sentences run as one masked launch (f_init.prefetch).  Results are those
-    of gen_sample sentence by sentence (the searches do not interact)."""
+    Every `chunk` consecutive sentences form one group: one masked encoder launch, then one device step advances the beams
+    of all of them (S = chunk sentences x k rows per f_next; see _DeviceBeam), so the decoder and readout weights are read
+    once per step for the whole group.  `concurrency` groups run interleaved, each on its own CUDA stream with its own
+    workspace.  Results are those of gen_sample sentence by sentence, in order (the sentences of a group do not interact).
+    Device memory per group in flight: see _DeviceBeam (3.7 GB at chunk = 16, beam 10, 100 steps, 800 source words,
+    dim 1000)."""
     eng = f_next.engine
     torch = eng.torch
     if k > 32 or getattr(f_init, 'device', None) is None or os.environ.get('NATS_DEVICE_BEAM', '1') == '0':
         return [gen_sample(tparams, f_init, f_next, numpy.asarray(x).reshape(-1, 1), options, trng, k, maxlen, False, False,
                            use_unk, kl_factor, ctx_factor, state_factor) for x in xs]
+    chunk = max(1, int(chunk))
     streams = getattr(eng, '_beam_streams', None)
     if streams is None:
         streams = eng._beam_streams = []
@@ -1326,21 +1372,19 @@ def gen_sample_many(tparams, f_init, f_next, xs, options, trng=None, k=5, maxlen
         streams.append(torch.cuda.Stream(device=eng.device))
     main = torch.cuda.current_stream(eng.device)
     results = [None] * len(xs)
-    nxt, parked_upto, active = 0, 0, {}
+    nxt, active = 0, {}
 
     def start(slot):
-        nonlocal nxt, parked_upto
-        if nxt >= parked_upto:
-            f_init.prefetch(xs[nxt:nxt + chunk])                  # on the current stream
-            parked_upto = nxt + chunk
-        streams[slot].wait_stream(main)                           # the encoder launch precedes the search that reads it
-        b = _DeviceBeam(f_init, f_next, numpy.asarray(xs[nxt]).reshape(-1, 1), k, maxlen, use_unk, kl_factor, ctx_factor,
-                        state_factor, None, slot + 1, streams[slot])
+        nonlocal nxt
+        grp = [numpy.asarray(x).reshape(-1) for x in xs[nxt:nxt + chunk]]
+        streams[slot].wait_stream(main)                           # whatever the current stream queued comes first
+        b = _DeviceBeam(f_init, f_next, grp, k, maxlen, use_unk, kl_factor, ctx_factor, state_factor, None, slot + 1,
+                        streams[slot])
         active[slot] = (nxt, b)
-        nxt += 1
+        nxt += len(grp)
         b.step()
 
-    for slot in range(min(concurrency, len(xs))):
+    for slot in range(min(concurrency, (len(xs) + chunk - 1) // chunk)):
         start(slot)
     while active:
         finished = []
@@ -1350,9 +1394,10 @@ def gen_sample_many(tparams, f_init, f_next, xs, options, trng=None, k=5, maxlen
                 finished.append((idx, b))
                 del active[slot]
                 if nxt < len(xs):
-                    start(slot)              # queued behind the finished search on the same stream (same workspace slot)
-        for idx, b in finished:              # fetching a result waits for that search only; the others have work queued
-            results[idx] = b.result()
+                    start(slot)              # queued behind the finished group on the same stream (same workspace slot)
+        for idx, b in finished:              # fetching a result waits for that group only; the others have work queued
+            res = b.result()
+            results[idx:idx + len(res)] = res
     return results
 
 
