@@ -374,14 +374,14 @@ int gemm_auto(const nats_ctx* ctx, cudaStream_t st, GemmProblem p, bool transA, 
     if (tc && p.batch == 1 && tiles >= ctx->num_sms && p.K >= 4096 && scratch != nullptr) {
         // deep products whose tile count is not a multiple of the SM count (d[U|Ux] of the encoder at dim 1000: 8 x 32 tiles
         // of 128 x 96, K = 12768, on 132 SMs): pick the split-K factor that minimises waves x (k-blocks per CTA + fixed cost)
-        // + the slab reduction.  The k-block cost is measured: that product unsplit took 1114 us for 2 waves of 399 k-blocks
-        // on an H100 80GB HBM3 at a 400 W power limit, i.e. 1.4 us per 128 x 96 x 32 k-block of 3xTF32.  The fixed cost per
-        // tile and the slab bandwidth (5 TB/s, L2-resident slabs) are estimates.
+        // + the slab reduction.  The k-block cost is measured: that product unsplit took 692-726 us for 2 waves of 399
+        // k-blocks on an H100 80GB HBM3 at a 700 W power limit, i.e. 0.9 us per 128 x 96 x 32 k-block of 3xTF32.  The fixed
+        // cost per tile and the slab bandwidth (5 TB/s, L2-resident slabs) are estimates.
         double best = 1e30;
         for (int s2 = 1; s2 <= 4; ++s2) {
             if ((long long)s2 * p.M * p.N > scratch_floats) break;
             const long long waves = (tiles * s2 + ctx->num_sms - 1) / ctx->num_sms;
-            double t = (double)waves * ((double)p.K / s2 / 32.0 * 1.4 + 3.0);
+            double t = (double)waves * ((double)p.K / s2 / 32.0 * 0.9 + 3.0);
             if (s2 > 1) t += (double)(s2 + 1) * p.M * p.N * 4.0 / 5.0e6;
             if (t < best) { best = t; splits = s2; }
         }

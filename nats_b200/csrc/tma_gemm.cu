@@ -252,20 +252,33 @@ __global__ void __launch_bounds__(kThreads, 1) tma_gemm_kernel(const __grid_cons
 // Non-skinny products (N side > 64): warp-specialized, persistent 128 x BN tiles (BN = 112 when the N side fits in one,
 // else 96: 1000 x 3000 takes 8 x 32 = 256 tiles, 1.94 waves of 132).
 //   warp 0 (one lane)  TMA producer: kWsNR raw stages of 32 k x (128 A rows | BN B rows) in flight, in the caller's layout.
-//                      The A box is 128-byte swizzled so that the consumers' fragment reads are (nearly) conflict-free.
-//   warps 1-3          split the raw B stage into K-major SWIZZLE_128B tf32 {hi, lo} tiles, a kWsNS-deep ring.
-//   warpgroups 1, 2    consumers, rows 64 (wg - 1) .. + 63: read their A fragments from the raw stage, split them in
-//                      registers and issue the register-A wgmma (m64nBNk8); one commit group per k-step, one in flight.
+//                      Both boxes are 128-byte swizzled where the source is K-major; the MN-major A box is loaded as four
+//                      swizzled 32-row boxes, so the consumers' fragment reads are (nearly) conflict-free.
+//   warps 1-3          tf32 split of the B stage into a kWsNS-deep ring of K-major SWIZZLE_128B tiles.  The tensor core
+//                      reads the upper 19 bits of an fp32 word, so the raw word is the hi operand and resid() the lo one:
+//                      a K-major B box is already the wgmma layout and the raw stage is B_hi, only B_lo is written; an
+//                      MN-major B box is transposed into a raw-word hi tile and a lo tile.
+//   warpgroups 1, 2    consumers, rows 64 (wg - 1) .. + 63: read their A fragments from the raw stage (hi = the word,
+//                      lo = its residual) and issue the register-A wgmma (m64nBNk8); one commit group per k-step, and
+//                      ws_in_flight<BN>() of them outstanding while the next k-step's fragments are read.
 // Stages are handed over by full / empty mbarrier pairs (no CTA barrier in the loop), so the producer and the split warps
-// run ahead into the next tile while the consumers store the current one.  The producer warpgroup gives registers to the
-// consumers (setmaxnreg 64 / 216), which hold the three accumulators of tma_gemm_kernel (3 x BN/2) beside the fragments of
-// two k-steps.  (At BN = 128 the three accumulators do not fit and ptxas serializes the wgmma; one accumulator for both
-// A_hi.B_hi halves loses accuracy at deep K.)  Per element the sums are those of tma_gemm_kernel in the same order, so a
-// product with the same split-K factor gives the same bits.
+// run ahead into the next tile while the consumers store the current one.  A consumer warpgroup frees a raw stage and its
+// split tile once the last MMA that reads them has retired.  The producer warpgroup gives registers to the consumers
+// (setmaxnreg 64 / 216), which hold the three accumulators of tma_gemm_kernel (3 x BN/2) beside the fragments of the
+// k-steps in flight.  (At BN = 128 the three accumulators do not fit and ptxas serializes the wgmma; one accumulator for
+// both A_hi.B_hi halves loses accuracy at deep K.)  Per element the sums are those of tma_gemm_kernel in the same order;
+// only the split of each operand differs (truncated hi, exact residual lo instead of rounded hi and lo).
 constexpr int kWsThreads = 384;
-constexpr int kWsNR = 4, kWsNS = 2;
+constexpr int kWsNR = 4, kWsNS = 3;
 template <int BN> __host__ __device__ constexpr uint32_t ws_raw() { return 128 * 128 + BN * 128; }    // raw stage: A 16 KB | B
-template <int BN> constexpr size_t ws_smem() { return (size_t)kWsNR * ws_raw<BN>() + (size_t)kWsNS * 2 * BN * 128 + 1024; }
+template <int BN, bool B_MN> __host__ __device__ constexpr uint32_t ws_split() { return (B_MN ? 2 : 1) * BN * 128; }
+template <int BN, bool B_MN> constexpr size_t ws_smem() {
+    return (size_t)kWsNR * ws_raw<BN>() + (size_t)kWsNS * ws_split<BN, B_MN>() + 1024;
+}
+// MMA k-steps a consumer warpgroup keeps outstanding.  The fragment registers form a ring of four sets indexed by the
+// k-step of the k-block (register arrays need compile-time indices); only ws_in_flight + 1 of them are live at a time.
+// At BN = 112 the accumulators take 168 registers and ptxas serializes the wgmma with a third live set: one in flight.
+template <int BN> __host__ __device__ constexpr int ws_in_flight() { return BN == 96 ? 2 : 1; }
 
 struct WsItem { int g, batch, split, m0, n0, kbeg, kend, nkb; };
 
@@ -294,10 +307,73 @@ __device__ __forceinline__ float raw_a_sw(uint32_t raw, int r, int k) {
     asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(raw + off));
     return v;
 }
+// raw B stage -> tf32 operand tiles, K-major SWIZZLE_128B.  K-major B (!MN) arrives swizzled: chunk q sits where wgmma
+// reads it, so only the residual is written, at the same offset.  MN-major B ([32 k][BN rows], unswizzled) is transposed
+// into a raw-word hi tile and a residual lo tile.  k past K reads as 0 (TMA fills out-of-bounds elements with zeros;
+// chunks of a K split are multiples of 32, so a k-block only ever crosses K itself).
+template <int BN, bool MN>
+__device__ __forceinline__ void split_b_ws(uint32_t raw, uint32_t hi_base, uint32_t lo_base, int tid) {
+    constexpr int kChunks = BN * 8, NT = 96;
+#pragma unroll
+    for (int i = 0; i < (kChunks + NT - 1) / NT; ++i) {
+        const int q = tid + i * NT;
+        if (q < kChunks) {
+            float4 v;
+            uint32_t off;
+            if (!MN) {
+                off = (uint32_t)q * 16u;
+                asm volatile("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(raw + off));
+            } else {                                          // a warp covers 32 consecutive rows: conflict-free reads
+                const int r = q % BN, c = q / BN;
+                v.x = raw_at<BN, true>(raw, r, 4 * c); v.y = raw_at<BN, true>(raw, r, 4 * c + 1);
+                v.z = raw_at<BN, true>(raw, r, 4 * c + 2); v.w = raw_at<BN, true>(raw, r, 4 * c + 3);
+                off = (uint32_t)(r * 128 + ((c ^ (r & 7)) << 4));
+                st_shared_v4(hi_base + off, v);
+            }
+            st_shared_v4(lo_base + off, make_float4(resid(v.x), resid(v.y), resid(v.z), resid(v.w)));
+        }
+    }
+}
 template <int N>
 __device__ __forceinline__ void reg_fence_u(uint32_t (&a)[N]) {
 #pragma unroll
     for (int i = 0; i < N; ++i) asm volatile("" : "+r"(a[i])::"memory");
+}
+
+// gemm_epilogue, with the two adjacent columns of each fragment pair stored as one float2 where the output rows are
+// contiguous and 8-byte aligned: a warp then writes whole 32-byte sectors (same value per element as gemm_epilogue)
+template <int R>
+__device__ __forceinline__ void ws_epilogue(const float (&acc0)[R], const float (&acc1)[R], const float (&accx)[R], float* C,
+                                            long long c_rs, long long c_cs, int Ma, int Nb, int rb, int cb,
+                                            const float* bias_a, const float* bias_n, bool accumulate) {
+    if (c_cs != 1 || (c_rs & 1) || (cb & 1) || (reinterpret_cast<uintptr_t>(C) & 7)) {
+        gemm_epilogue(acc0, acc1, accx, C, c_rs, c_cs, Ma, Nb, rb, cb, bias_a, bias_n, accumulate);
+        return;
+    }
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        const int i_row = rb + 8 * h;
+        if (i_row >= Ma) continue;
+        const float ba = bias_a ? __ldg(bias_a + i_row) : 0.f;
+        float* crow = C + (long long)i_row * c_rs;
+#pragma unroll
+        for (int j = 0; j < R / 4; ++j) {
+            const int idx = 4 * j + 2 * h, col = cb + 8 * j;
+            if (col >= Nb) continue;
+            float o0 = (acc0[idx] + acc1[idx]) + accx[idx] + ba;
+            float o1 = (acc0[idx + 1] + acc1[idx + 1]) + accx[idx + 1] + ba;
+            if (col + 1 < Nb) {
+                if (bias_n) { o0 += __ldg(bias_n + col); o1 += __ldg(bias_n + col + 1); }
+                float2* cp = reinterpret_cast<float2*>(crow + col);
+                if (accumulate) { const float2 c = *cp; o0 += c.x; o1 += c.y; }
+                *cp = make_float2(o0, o1);
+            } else {
+                if (bias_n) o0 += __ldg(bias_n + col);
+                if (accumulate) o0 += crow[col];
+                crow[col] = o0;
+            }
+        }
+    }
 }
 
 template <int BN>
@@ -308,9 +384,10 @@ __device__ __forceinline__ void mma_rs_ws(float (&d)[BN / 2], const uint32_t (&a
 
 template <int BN, bool A_MN, bool B_MN>
 __global__ void __launch_bounds__(kWsThreads, 1) tma_gemm_kernel_ws(const __grid_constant__ TmaGroup grp, int items) {
-    constexpr uint32_t kRaw = ws_raw<BN>(), kBHalf = BN * 128, kSplit = 2 * kBHalf;
-    constexpr int R = BN / 2;
+    constexpr uint32_t kRaw = ws_raw<BN>(), kBHalf = BN * 128, kSplit = ws_split<BN, B_MN>();
+    constexpr int R = BN / 2, kIF = ws_in_flight<BN>();
     static_assert(BN == 96 || BN == 112, "BN");
+    static_assert(kIF >= 1 && kIF <= 3, "the fragment ring holds four k-steps");
     extern __shared__ __align__(1024) unsigned char smem[];
     __shared__ __align__(8) uint64_t full[kWsNR], empty[kWsNR], sfull[kWsNS], sempty[kWsNS];
     // the warp index as a shuffled (provably warp-uniform) value: role branches on it do not serialize the wgmma inside them
@@ -323,7 +400,7 @@ __global__ void __launch_bounds__(kWsThreads, 1) tma_gemm_kernel_ws(const __grid
             asm volatile("prefetch.tensormap [%0];" ::"l"(&grp.mapA[g]) : "memory");
             asm volatile("prefetch.tensormap [%0];" ::"l"(&grp.mapB[g]) : "memory");
         }
-        for (int s = 0; s < kWsNR; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 3 + 8); }   // split warps + consumer warps
+        for (int s = 0; s < kWsNR; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 3 + 2); }   // split warps + consumer warpgroups
         for (int s = 0; s < kWsNS; ++s) { mbar_init(&sfull[s], 3); mbar_init(&sempty[s], 2); }    // split warps / consumer warpgroups
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
@@ -366,8 +443,7 @@ __global__ void __launch_bounds__(kWsThreads, 1) tma_gemm_kernel_ws(const __grid
                     mbar_wait(&full[s], (kc / kWsNR) & 1);
                     mbar_wait(&sempty[t], ((kc / kWsNS) & 1) ^ 1);
                     const uint32_t sp = split_base + (uint32_t)t * kSplit;
-                    split_tile<BN, B_MN, 96>(smem_base + (uint32_t)s * kRaw + 128 * 128, sp, sp + kBHalf,
-                                              w.kend - (w.kbeg + kb * kBlockK), stid);
+                    split_b_ws<BN, B_MN>(smem_base + (uint32_t)s * kRaw + 128 * 128, sp, B_MN ? sp + kBHalf : sp, stid);
                     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> wgmma
                     __syncwarp();
                     if (lane == 0) { mbar_arrive(&sfull[t]); mbar_arrive(&empty[s]); }
@@ -388,48 +464,51 @@ __global__ void __launch_bounds__(kWsThreads, 1) tma_gemm_kernel_ws(const __grid
         float acc0[R], acc1[R], accx[R];
 #pragma unroll
         for (int i = 0; i < R; ++i) { acc0[i] = 0.f; acc1[i] = 0.f; accx[i] = 0.f; }
-        uint32_t fa[2][2][4] = {};       // [k-step parity][hi, lo][fragment]: the registers of the MMAs in flight
+        uint32_t fa[4][2][4] = {};       // [k-step][hi, lo][fragment]: the registers of the MMAs in flight
         for (int kb = 0; kb < w.nkb; ++kb, ++kc) {
             const int s = kc % kWsNR, t = kc % kWsNS;
             mbar_wait(&full[s], (kc / kWsNR) & 1);
             mbar_wait(&sfull[t], (kc / kWsNS) & 1);
             const uint32_t raw = smem_base + (uint32_t)s * kRaw;
             const uint32_t sp = split_base + (uint32_t)t * kSplit;
-            const uint64_t b_hi = desc_sw128(sp), b_lo = desc_sw128(sp + kBHalf);
+            const uint64_t b_hi = desc_sw128(B_MN ? sp : raw + 128 * 128), b_lo = desc_sw128(B_MN ? sp + kBHalf : sp);
 #pragma unroll
             for (int kk = 0; kk < 4; ++kk) {
-                uint32_t (&ah)[4] = fa[kk & 1][0];
-                uint32_t (&al)[4] = fa[kk & 1][1];
+                uint32_t (&ah)[4] = fa[kk][0];
+                uint32_t (&al)[4] = fa[kk][1];
                 // k beyond the chunk end only occurs at K itself (chunks are multiples of 32), which TMA fills with zeros
 #pragma unroll
                 for (int f = 0; f < 4; ++f) {
                     const float x = raw_a_sw<A_MN>(raw, r0 + 8 * (f & 1), 8 * kk + q + 4 * (f >> 1));
-                    const float h = to_tf32(x);
-                    ah[f] = __float_as_uint(h);
-                    al[f] = __float_as_uint(to_tf32(x - h));
-                }
-                if (kk == 3) {           // this warp is done reading raw stage s
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(&empty[s]);
+                    ah[f] = __float_as_uint(x);
+                    al[f] = __float_as_uint(resid(x));
                 }
                 wgmma_fence();
                 mma_rs_ws<BN>(accx, al, b_hi + 2 * kk);
                 mma_rs_ws<BN>(accx, ah, b_lo + 2 * kk);
                 mma_rs_ws<BN>((kk & 1) ? acc1 : acc0, ah, b_hi + 2 * kk);
                 wgmma_commit();
-                wgmma_wait<1>();         // the previous k-step has retired: its fragment registers may be rewritten
-                reg_fence_u(fa[(kk + 1) & 1][0]); reg_fence_u(fa[(kk + 1) & 1][1]);
-                if (kk == 0 && kb > 0 && (ctid & 127) == 0) mbar_arrive(&sempty[(kc - 1) % kWsNS]);
+                wgmma_wait<kIF>();       // k-step kk - kIF has retired: its fragment registers may be rewritten
+                reg_fence_u(fa[(kk + 4 - kIF) & 3][0]); reg_fence_u(fa[(kk + 4 - kIF) & 3][1]);
+                // k-step 3 of the previous k-block has retired: its raw stage and split tile are free
+                if (kk == kIF - 1 && kb > 0 && (ctid & 127) == 0) {
+                    mbar_arrive(&empty[(kc - 1) % kWsNR]);
+                    mbar_arrive(&sempty[(kc - 1) % kWsNS]);
+                }
             }
         }
         wgmma_wait<0>();
         reg_fence(acc0); reg_fence(acc1); reg_fence(accx);
-        reg_fence_u(fa[0][0]); reg_fence_u(fa[0][1]); reg_fence_u(fa[1][0]); reg_fence_u(fa[1][1]);
-        if (w.nkb > 0 && (ctid & 127) == 0) mbar_arrive(&sempty[(kc - 1) % kWsNS]);
+#pragma unroll
+        for (int j = 0; j < 4; ++j) { reg_fence_u(fa[j][0]); reg_fence_u(fa[j][1]); }
+        if (w.nkb > 0 && (ctid & 127) == 0) {
+            mbar_arrive(&empty[(kc - 1) % kWsNR]);
+            mbar_arrive(&sempty[(kc - 1) % kWsNS]);
+        }
         const bool add_bias = (P.bias != nullptr) && (w.split == 0);
-        gemm_epilogue(acc0, acc1, accx, P.C + (long long)w.batch * P.sC + (long long)w.split * P.strideP, P.c_rs, P.c_cs, P.Ma,
-                      P.Nb, w.m0 + r0, w.n0 + 2 * q, (add_bias && P.bias_on_a) ? P.bias : nullptr,
-                      (add_bias && !P.bias_on_a) ? P.bias : nullptr, P.accumulate != 0);
+        ws_epilogue(acc0, acc1, accx, P.C + (long long)w.batch * P.sC + (long long)w.split * P.strideP, P.c_rs, P.c_cs, P.Ma,
+                    P.Nb, w.m0 + r0, w.n0 + 2 * q, (add_bias && P.bias_on_a) ? P.bias : nullptr,
+                    (add_bias && !P.bias_on_a) ? P.bias : nullptr, P.accumulate != 0);
     }
 }
 
@@ -507,13 +586,19 @@ int operand_map_ws_a(const float* ptr, bool mn, int rows, int K, int ld, int bat
     const long long d0 = mn ? rows : K, d1 = mn ? K : rows;
     return encode_tile3d(ptr, d0, d1, batch, ld, batch > 1 ? bstride : d1 * ld, 32, mn ? 32 : 128, 1, true, out);
 }
+// BN side of tma_gemm_kernel_ws: K-major source -> box (32 k, BN rows) 128-byte swizzled, i.e. the K-major SWIZZLE_128B
+// layout wgmma reads; MN-major source -> box (BN rows, 32 k), unswizzled, transposed by the split warps
+int operand_map_ws_b(const float* ptr, bool mn, int rows, int K, int ld, int batch, long long bstride, int bn, CUtensorMap* out) {
+    if (mn) return operand_map(ptr, true, rows, K, ld, batch, bstride, bn, out);
+    return encode_tile3d(ptr, K, rows, batch, ld, batch > 1 ? bstride : rows * (long long)ld, 32, bn, 1, true, out);
+}
 
 template <int BN>
 int set_attrs_ws() {
-    const int sm = (int)ws_smem<BN>();
-    NATS_CUDA_OK(cudaFuncSetAttribute(tma_gemm_kernel_ws<BN, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, sm));
+    const int sk = (int)ws_smem<BN, false>(), sm = (int)ws_smem<BN, true>();
+    NATS_CUDA_OK(cudaFuncSetAttribute(tma_gemm_kernel_ws<BN, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, sk));
     NATS_CUDA_OK(cudaFuncSetAttribute(tma_gemm_kernel_ws<BN, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, sm));
-    NATS_CUDA_OK(cudaFuncSetAttribute(tma_gemm_kernel_ws<BN, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, sm));
+    NATS_CUDA_OK(cudaFuncSetAttribute(tma_gemm_kernel_ws<BN, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, sk));
     NATS_CUDA_OK(cudaFuncSetAttribute(tma_gemm_kernel_ws<BN, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, sm));
     return 0;
 }
@@ -521,7 +606,7 @@ int set_attrs_ws() {
 template <int BN>
 int launch_ws(cudaStream_t st, const TmaGroup& grp, bool a_mn, bool b_mn, int items) {
     const dim3 grid(min(items, g_num_sms)), block(kWsThreads);     // persistent: one CTA per SM at most
-    const size_t sm = ws_smem<BN>();
+    const size_t sm = b_mn ? ws_smem<BN, true>() : ws_smem<BN, false>();
     cudaError_t e;
     if (!a_mn && !b_mn) e = launch_pdl(tma_gemm_kernel_ws<BN, false, false>, grid, block, sm, st, grp, items);
     else if (!a_mn && b_mn) e = launch_pdl(tma_gemm_kernel_ws<BN, false, true>, grid, block, sm, st, grp, items);
@@ -602,9 +687,13 @@ int tma_gemm_launch(cudaStream_t st, const GemmProblem* probs, int count, bool t
         const int rows_a = swapped ? q.N : q.M, rows_b = swapped ? q.M : q.N;
         const int ld_a = swapped ? q.ldb : q.lda, ld_b = swapped ? q.lda : q.ldb;
         const long long s_a = swapped ? q.strideB : q.strideA, s_b = swapped ? q.strideA : q.strideB;
-        if (skinny) NATS_TRY(operand_map(pa, a_mn, rows_a, q.K, ld_a, q.batch, s_a, 128, &grp.mapA[i]));
-        else NATS_TRY(operand_map_ws_a(pa, a_mn, rows_a, q.K, ld_a, q.batch, s_a, &grp.mapA[i]));
-        NATS_TRY(operand_map(pb, b_mn, rows_b, q.K, ld_b, q.batch, s_b, BN, &grp.mapB[i]));
+        if (skinny) {
+            NATS_TRY(operand_map(pa, a_mn, rows_a, q.K, ld_a, q.batch, s_a, 128, &grp.mapA[i]));
+            NATS_TRY(operand_map(pb, b_mn, rows_b, q.K, ld_b, q.batch, s_b, BN, &grp.mapB[i]));
+        } else {
+            NATS_TRY(operand_map_ws_a(pa, a_mn, rows_a, q.K, ld_a, q.batch, s_a, &grp.mapA[i]));
+            NATS_TRY(operand_map_ws_b(pb, b_mn, rows_b, q.K, ld_b, q.batch, s_b, BN, &grp.mapB[i]));
+        }
         t.Ma = rows_a; t.Nb = rows_b;
         if (!swapped) { t.c_rs = q.ldc; t.c_cs = 1; t.bias_on_a = 0; }
         else { t.c_rs = 1; t.c_cs = q.ldc; t.bias_on_a = 1; }
