@@ -119,7 +119,9 @@ int nats_encoder_bwd(nats_ctx_t* ctx, void* stream, const nats_dims_t* dims, con
                      void* ws, int64_t ws_bytes, float* grads);
 
 /* Read-only views into a training workspace (for tests / alignment dumps): name in
- * {"ctx","init_state","dec_h","dec_ctx","dec_alpha","pctx","logits"}; returns device pointer or NULL. */
+ * {"ctx","init_state","dec_h","dec_ctx","dec_alpha","pctx","logits","dcc","dmean"}; returns device pointer or NULL.
+ * "dcc" [Tx,B,2D] = d cost / d ctx from the decoder and "dmean" [B,2D] = d cost / d ctx_mean (not yet divided by the
+ * source length): the gradient the encoder backward reads, valid after nats_train_bwd_begin. */
 const float* nats_train_ws_view(const nats_dims_t* dims, int Tx, int Ty, int B, void* ws, const char* name);
 
 /* ---------------------------------------------------------------- sampler graph (build_sampler) ---- */

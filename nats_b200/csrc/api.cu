@@ -338,6 +338,8 @@ const float* nats_train_ws_view(const nats_dims_t* dims, int Tx, int Ty, int B, 
     if (!strcmp(name, "dec_alpha")) return w.d_alpha;
     if (!strcmp(name, "pctx")) return w.pctx;
     if (!strcmp(name, "logits")) return w.logits;
+    if (!strcmp(name, "dcc")) return w.dcc;
+    if (!strcmp(name, "dmean")) return w.dmean;
     return nullptr;
 }
 
