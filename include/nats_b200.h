@@ -275,12 +275,24 @@ int nats_beam_step(nats_ctx_t* ctx, void* stream, const nats_dims_t* dims, const
  *     hypotheses in slots [0, counters[8*s + 3]);
  *   host_counters (NULL = off): page-locked host memory, int32[8]; [5] receives the number of sentences that are done
  *     (for S = 1 also words 0..4), so the host polls one flag for the whole group.
- * A sentence that is done stays untouched while the others go on.  Errors: k < 1 or k > 32, S < 1, NULL src_len or
- * buffers. */
+ * A sentence that is done stays untouched while the others go on.
+ * Output constraints (additions beyond the reference; 0 = off, and with both 0 the step is exactly the one above).  At
+ * step ii a live row holds the words y_0 .. y_{ii-1} (no BOS, no EOS), and its next-word probabilities are changed before
+ * the per-row top-k:
+ *   no_repeat_ngram = N >= 1: for every j in [0, ii-N] with y_j .. y_{j+N-2} == y_{ii-N+1} .. y_{ii-1}, word y_{j+N-1}
+ *     gets probability 0 (N = 1: every word already in the row), so no hypothesis contains the same N-gram twice;
+ *   min_len = L: while ii < L, word 0 (EOS) gets probability 0, so every retired hypothesis has >= L words before EOS.
+ *   With use_unk == 0, entry 1 is set to 1e-20 first, so a banned UNK gets 0.  A banned word's candidate cost is +inf,
+ *   like a word whose probability underflows; scores and the distraction re-ranking are otherwise unchanged.  A row with
+ *   fewer than k admissible words may still select +inf candidates.  The constraints act on beam search only.
+ * Errors: k < 1 or k > 32, S < 1, NULL src_len or buffers, no_repeat_ngram < 0 or min_len < 0, a constraint on with
+ * maxlen > 12288. */
 typedef struct nats_beam_step_many {
     nats_beam_step_t beam;               /* Tx = longest source, k = rows per sentence */
     int32_t n_src;                       /* S */
     const int32_t* src_len;              /* [S] device */
+    int32_t no_repeat_ngram;             /* N: block repeated N-grams (0 = off) */
+    int32_t min_len;                     /* L: no EOS before L words (0 = off) */
 } nats_beam_step_many_t;
 int nats_beam_step_many(nats_ctx_t* ctx, void* stream, const nats_dims_t* dims, const nats_beam_step_many_t* a, int step);
 

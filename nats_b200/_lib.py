@@ -40,8 +40,8 @@ class BeamStep(Structure):
 
 
 class BeamStepMany(Structure):
-    """nats_beam_step_many_t of include/nats_b200.h: a group of n_src sentences x k rows"""
-    _fields_ = [('beam', BeamStep), ('n_src', c_int32), ('src_len', _P)]
+    """nats_beam_step_many_t of include/nats_b200.h: a group of n_src sentences x k rows, with the output constraints"""
+    _fields_ = [('beam', BeamStep), ('n_src', c_int32), ('src_len', _P), ('no_repeat_ngram', c_int32), ('min_len', c_int32)]
 
 # name -> (restype, argtypes); mirrors include/nats_b200.h one to one (checked by tests/test_abi.py)
 SIGNATURES = {

@@ -75,7 +75,7 @@ struct ViewDef { const char* name; int64_t off; int rows, cols, ld, ndim; };
 extern "C" {
 
 const char* nats_last_error(void) { return g_err; }
-int nats_version(void) { return 101; }
+int nats_version(void) { return 102; }
 
 int nats_ctx_create(int device, nats_ctx_t** out) {
     NATS_REQUIRE(out != nullptr, "out");
@@ -570,9 +570,10 @@ namespace {
 
 // One beam step of a group of n_src sentences x k rows (nats.py:957-1066 for each sentence): f_next on all rows, each
 // attending to its own source (ctx [Tx, n_src, C]; n_src = 1 with src_len NULL is the single-sentence layout [Tx, C]),
-// distraction scores of the live rows, per-row top-k, one selection warp per sentence, one gather launch.
+// distraction scores of the live rows, the output constraints when one is on, per-row top-k, one selection warp per
+// sentence, one gather launch.
 int beam_step_group(nats_ctx_t* ctx, cudaStream_t st, const nats_dims_t* dims, const nats_beam_step_t* a, int n_src,
-                    const int32_t* src_len, int step) {
+                    const int32_t* src_len, int no_repeat_ngram, int min_len, int step) {
     NATS_REQUIRE(ctx && dims && a, "null argument");
     NATS_REQUIRE(a->k >= 1 && a->k <= 32 && a->maxlen >= 1 && step >= 0 && step < a->maxlen, "beam step shape (1 <= k <= 32)");
     NATS_REQUIRE(n_src >= 1 && (long long)n_src * a->k <= 65535, "beam group size");
@@ -596,7 +597,13 @@ int beam_step_group(nats_ctx_t* ctx, cudaStream_t st, const nats_dims_t* dims, c
     NATS_REQUIRE(a->state_next && a->acc_ctx_next && a->acc_alpha_next && a->hist_alpha_in && a->hist_alpha_out && a->out_alpha,
                  "null argument");
     NATS_REQUIRE(!distract || (a->hist_ctx_out && a->hist_state_out), "distraction histories");
-    NATS_TRY(beam_topk(st, a->probs, n, V, k, a->use_unk ? 0 : 1, a->top_p, a->top_i));
+    int mask_unk = a->use_unk ? 0 : 1;
+    if (no_repeat_ngram > 0 || min_len > 0) {                         // the UNK mask moves into the constraint kernel
+        NATS_TRY(beam_constrain(st, a->probs, V, a->tokens, a->maxlen, step, n_src, k, a->counters, no_repeat_ngram, min_len,
+                                mask_unk));
+        mask_unk = 0;
+    }
+    NATS_TRY(beam_topk(st, a->probs, n, V, k, mask_unk, a->top_p, a->top_i));
     NATS_TRY(beam_select(st, a->top_p, a->top_i, use_pen ? a->pen : nullptr, n_src, k, a->maxlen, step, a->counters, a->scores,
                          a->tokens, a->parents, reinterpret_cast<long long*>(const_cast<int64_t*>(a->next_w)), a->out_tokens,
                          a->out_len, a->out_score, a->fin_parent, a->host_counters));
@@ -612,14 +619,18 @@ int beam_step_group(nats_ctx_t* ctx, cudaStream_t st, const nats_dims_t* dims, c
 extern "C" {
 
 int nats_beam_step(nats_ctx_t* ctx, void* stream, const nats_dims_t* dims, const nats_beam_step_t* a, int step) {
-    return beam_step_group(ctx, reinterpret_cast<cudaStream_t>(stream), dims, a, 1, nullptr, step);
+    return beam_step_group(ctx, reinterpret_cast<cudaStream_t>(stream), dims, a, 1, nullptr, 0, 0, step);
 }
 
 int nats_beam_step_many(nats_ctx_t* ctx, void* stream, const nats_dims_t* dims, const nats_beam_step_many_t* a, int step) {
     NATS_REQUIRE(a != nullptr, "null argument");
     NATS_REQUIRE(a->n_src >= 1, "n_src >= 1");
     NATS_REQUIRE(a->src_len != nullptr, "src_len");
-    return beam_step_group(ctx, reinterpret_cast<cudaStream_t>(stream), dims, &a->beam, a->n_src, a->src_len, step);
+    NATS_REQUIRE(a->no_repeat_ngram >= 0 && a->min_len >= 0, "no_repeat_ngram and min_len must be >= 0");
+    NATS_REQUIRE((a->no_repeat_ngram == 0 && a->min_len == 0) || a->beam.maxlen <= kBeamConstrainMaxLen,
+                 "no_repeat_ngram / min_len need maxlen <= 12288");
+    return beam_step_group(ctx, reinterpret_cast<cudaStream_t>(stream), dims, &a->beam, a->n_src, a->src_len,
+                           a->no_repeat_ngram, a->min_len, step);
 }
 
 

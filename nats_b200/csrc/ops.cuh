@@ -196,6 +196,11 @@ int beam_distraction_scores(cudaStream_t st, const float* hist_alpha, const floa
 int beam_topk(cudaStream_t st, const float* probs, int n, int V, int K, int mask_unk, float* out_p, int32_t* out_idx);
 int beam_reorder_append(cudaStream_t st, const float* src, float* dst, const float* cur, const int32_t* parent,
                         int n_new, int len_cap, int hist_len, int dim);
+// n-gram blocking and minimum length on the live rows' probs [n_src*k, V] before beam_topk (tokens: beam_select's ping-pong
+// [2, n_src*k, maxlen] histories, read at parity step & 1); entry 1 = 1e-20 first when mask_unk: see ops_beam.cu
+constexpr int kBeamConstrainMaxLen = 12288;   // a row's history is staged in (at most 48 KB of) shared memory
+int beam_constrain(cudaStream_t st, float* probs, int V, const int32_t* tokens, int maxlen, int step, int n_src, int k,
+                   const int32_t* counters, int no_repeat, int min_len, int mask_unk);
 // device-resident bookkeeping of one beam step (nats.py:976-1066) for a group of n_src sentences x k rows: see ops_beam.cu
 int beam_select(cudaStream_t st, const float* top_p, const int32_t* top_i, const float* pen, int n_src, int k, int maxlen,
                 int step, int32_t* counters, float* scores, int32_t* tokens, int32_t* parents, long long* next_w,

@@ -307,7 +307,47 @@ __global__ void __launch_bounds__(256) beam_advance_kernel(const __grid_constant
     }
 }
 
+// Output constraints on the next-word probabilities of the live rows (an addition beyond the reference), one warp per row
+// of the group.  Row r holds `step` words in tokens[r] (tokens = the current parity's [n, maxlen] rows).  With
+// no_repeat = N >= 1, for every start j in [0, step - N] whose N-1 words equal the row's last N-1 words, word
+// tokens[r][j + N - 1] gets probability 0: no hypothesis contains an N-gram twice.  While step < min_len, word 0 (EOS)
+// gets probability 0.  mask_unk writes entry 1 = 1e-20 (nats.py:975) BEFORE the bans, so a banned UNK ends at 0.
+__global__ void __launch_bounds__(32) beam_constrain_kernel(float* __restrict__ probs, int V, const int32_t* __restrict__ tokens,
+                                                            int maxlen, int step, int k, const int32_t* __restrict__ counters,
+                                                            int no_repeat, int min_len, int mask_unk) {
+    extern __shared__ int32_t s_hist[];                               // the row's `step` words
+    const int row = blockIdx.x, lane = threadIdx.x;
+    if (beam_row_idle(counters, k, row)) return;
+    float* p = probs + (long long)row * V;
+    const int32_t* tk = tokens + (long long)row * maxlen;
+    for (int t = lane; t < step; t += 32) s_hist[t] = tk[t];
+    if (mask_unk && lane == 0) p[1] = 1e-20f;
+    __syncwarp();                                                     // orders the history and the UNK store before the bans
+    if (step < min_len && lane == 0) p[0] = 0.f;
+    if (no_repeat < 1 || step < no_repeat) return;
+    const int sfx = step - no_repeat + 1;                             // first word of the row's (N-1)-word suffix
+    for (int j = lane; j < sfx; j += 32) {
+        bool hit = true;
+        for (int q = 0; q < no_repeat - 1 && hit; ++q) hit = s_hist[j + q] == s_hist[sfx + q];
+        const int w = s_hist[j + no_repeat - 1];
+        if (hit && w >= 0 && w < V) p[w] = 0.f;                       // several lanes may ban the same word: same store
+    }
+}
+
 }  // namespace
+
+int beam_constrain(cudaStream_t st, float* probs, int V, const int32_t* tokens, int maxlen, int step, int n_src, int k,
+                   const int32_t* counters, int no_repeat, int min_len, int mask_unk) {
+    NATS_REQUIRE(k >= 1 && n_src >= 1 && (long long)n_src * k <= 65535 && step >= 0 && step < maxlen, "beam_constrain shape");
+    NATS_REQUIRE(no_repeat >= 0 && min_len >= 0, "beam constraints must be >= 0");
+    NATS_REQUIRE(maxlen <= kBeamConstrainMaxLen, "beam constraints need maxlen <= 12288");
+    const int n = n_src * k;
+    ProfScope ps(st, K_BEAM);
+    beam_constrain_kernel<<<n, 32, (size_t)step * sizeof(int32_t), st>>>(probs, V, tokens + (long long)(step & 1) * n * maxlen,
+                                                                      maxlen, step, k, counters, no_repeat, min_len, mask_unk);
+    NATS_LAUNCH_OK();
+    return 0;
+}
 
 int beam_select(cudaStream_t st, const float* top_p, const int32_t* top_i, const float* pen, int n_src, int k, int maxlen,
                 int step, int32_t* counters, float* scores, int32_t* tokens, int32_t* parents, long long* next_w,

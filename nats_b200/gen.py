@@ -4,6 +4,9 @@ score).  The reference spreads sentences over `-p` CPU processes; here `-p` work
 the visible GPUs (one model replica per process, gen.py:78-85) and `-p 1` decodes in-process.
 
     python -m nats_b200.gen -n -p 8 -k 5 -l KL -x CTX -s STATE model.npz dictionary.pkl source.txt out.txt
+
+Two long options go beyond the reference, both off by default: `--no-repeat-ngram N` keeps every summary free of a repeated
+N-gram and `--min-len L` lets no summary end before L words (nats.gen_sample's no_repeat_ngram / min_len).
 """
 import argparse
 import multiprocessing as mp
@@ -28,7 +31,7 @@ CHUNK = 16     # sentences encoded per f_init launch (and per queue item of a wo
 class _Translator(object):
     """one model replica: parameters from the checkpoint, sampler, beam search (gen.py:15-48)"""
 
-    def __init__(self, model, options, k, normalize, kl_factor, ctx_factor, state_factor):
+    def __init__(self, model, options, k, normalize, kl_factor, ctx_factor, state_factor, no_repeat_ngram=0, min_len=0):
         from . import nats
         self.nats = nats
         params = nats.load_params(model, nats.init_params(options))
@@ -36,6 +39,7 @@ class _Translator(object):
         self.f_init, self.f_next = nats.build_sampler(self.tparams, options, None)
         self.options, self.k, self.normalize = options, k, normalize
         self.factors = (kl_factor, ctx_factor, state_factor)
+        self.constraints = dict(no_repeat_ngram=no_repeat_ngram, min_len=min_len)
 
     def prefetch(self, seqs):
         """encode the next sentences in ONE encoder launch (f_init is most of a short summary's time); optional"""
@@ -49,7 +53,7 @@ class _Translator(object):
         outs = self.nats.gen_sample_many(self.tparams, self.f_init, self.f_next, [numpy.array(s, dtype='int64') for s in seqs],
                                          self.options, trng=None, k=self.k, maxlen=100, use_unk=True, kl_factor=kl,
                                          ctx_factor=cf, state_factor=sf, concurrency=int(os.environ.get('NATS_GEN_STREAMS', '12')),
-                                         chunk=CHUNK)
+                                         chunk=CHUNK, **self.constraints)
         return [self._best(*o) for o in outs]
 
     def __call__(self, seq):
@@ -57,7 +61,7 @@ class _Translator(object):
         sample, score, alphas = self.nats.gen_sample(
             self.tparams, self.f_init, self.f_next, numpy.array(seq, dtype='int64').reshape([len(seq), 1]), self.options,
             trng=None, k=self.k, maxlen=100, stochastic=False, argmax=False, use_unk=True, kl_factor=kl, ctx_factor=cf,
-            state_factor=sf)
+            state_factor=sf, **self.constraints)
         return self._best(sample, score, alphas)
 
     def _best(self, sample, score, alphas):
@@ -69,12 +73,13 @@ class _Translator(object):
         return [int(w) for w in sample[sidx]], align_pos
 
 
-def translate_model(queue, rqueue, pid, model, options, k, normalize, kl_factor, ctx_factor, state_factor):
+def translate_model(queue, rqueue, pid, model, options, k, normalize, kl_factor, ctx_factor, state_factor, no_repeat_ngram=0,
+                    min_len=0):
     import torch
     n_dev = max(torch.cuda.device_count(), 1)
     os.environ['LOCAL_RANK'] = str(pid % n_dev)               # the engine binds to this device
     torch.cuda.set_device(pid % n_dev)
-    tr = _Translator(model, options, k, normalize, kl_factor, ctx_factor, state_factor)
+    tr = _Translator(model, options, k, normalize, kl_factor, ctx_factor, state_factor, no_repeat_ngram, min_len)
     while True:
         req = queue.get()
         if req is None:
@@ -85,7 +90,9 @@ def translate_model(queue, rqueue, pid, model, options, k, normalize, kl_factor,
 
 
 def main(model, dictionary, source_file, saveto, k=5, normalize=False, n_process=5, chr_level=False, kl_factor=0,
-         ctx_factor=0, state_factor=0):
+         ctx_factor=0, state_factor=0, no_repeat_ngram=0, min_len=0):
+    if no_repeat_ngram < 0 or min_len < 0:
+        raise ValueError('--no-repeat-ngram and --min-len must be >= 0 (0 = off)')
     options = _load_pickle('%s.pkl' % model)
     word_dict = _load_pickle(dictionary)
     word_idict = dict((vv, kk) for kk, vv in word_dict.items())
@@ -105,7 +112,7 @@ def main(model, dictionary, source_file, saveto, k=5, normalize=False, n_process
     print('Inferece ', source_file, '...')
     trans, pos = [None] * n_samples, [None] * n_samples
     if n_process <= 1:
-        tr = _Translator(model, options, k, normalize, kl_factor, ctx_factor, state_factor)
+        tr = _Translator(model, options, k, normalize, kl_factor, ctx_factor, state_factor, no_repeat_ngram, min_len)
         for lo in range(0, len(jobs), CHUNK):
             for (idx, _), (seq, p_) in zip(jobs[lo:lo + CHUNK], tr.many([j[1] for j in jobs[lo:lo + CHUNK]])):
                 trans[idx], pos[idx] = seq, p_
@@ -114,7 +121,8 @@ def main(model, dictionary, source_file, saveto, k=5, normalize=False, n_process
         ctx = mp.get_context('spawn')                          # CUDA contexts do not survive fork
         queue, rqueue = ctx.Queue(), ctx.Queue()
         procs = [ctx.Process(target=translate_model, args=(queue, rqueue, midx, model, options, k, normalize, kl_factor,
-                                                           ctx_factor, state_factor)) for midx in range(n_process)]
+                                                           ctx_factor, state_factor, no_repeat_ngram, min_len))
+                 for midx in range(n_process)]
         for p in procs:
             p.start()
         for lo in range(0, len(jobs), CHUNK):
@@ -152,10 +160,15 @@ if __name__ == '__main__':
     parser.add_argument('-s', type=float, default=0)
     parser.add_argument('-n', action='store_true', default=False)
     parser.add_argument('-c', action='store_true', default=False)
+    parser.add_argument('--no-repeat-ngram', type=int, default=0, metavar='N',
+                        help='no summary contains the same N-gram twice (0 = off)')
+    parser.add_argument('--min-len', type=int, default=0, metavar='L',
+                        help='no summary ends before L words (0 = off)')
     parser.add_argument('model', type=str)
     parser.add_argument('dictionary', type=str)
     parser.add_argument('source', type=str)
     parser.add_argument('saveto', type=str)
     args = parser.parse_args()
     main(args.model, args.dictionary, args.source, args.saveto, k=args.k, normalize=args.n, n_process=args.p,
-         chr_level=args.c, kl_factor=args.l, ctx_factor=args.x, state_factor=args.s)
+         chr_level=args.c, kl_factor=args.l, ctx_factor=args.x, state_factor=args.s, no_repeat_ngram=args.no_repeat_ngram,
+         min_len=args.min_len)

@@ -1156,13 +1156,15 @@ class _DeviceBeam(object):
     it 3.2 GB."""
 
     def __init__(self, f_init, f_next, xs, k, maxlen, use_unk, kl_factor, ctx_factor, state_factor, _trace=None, slot=0,
-                 stream=None):
+                 stream=None, no_repeat_ngram=0, min_len=0):
         torch = f_next.engine.torch
         self.tstream = stream if stream is not None else torch.cuda.current_stream(f_next.engine.device)
         with torch.cuda.stream(self.tstream):
-            self._setup(f_init, f_next, xs, k, maxlen, use_unk, kl_factor, ctx_factor, state_factor, _trace, slot)
+            self._setup(f_init, f_next, xs, k, maxlen, use_unk, kl_factor, ctx_factor, state_factor, _trace, slot,
+                        no_repeat_ngram, min_len)
 
-    def _setup(self, f_init, f_next, xs, k, maxlen, use_unk, kl_factor, ctx_factor, state_factor, _trace, slot):
+    def _setup(self, f_init, f_next, xs, k, maxlen, use_unk, kl_factor, ctx_factor, state_factor, _trace, slot,
+               no_repeat_ngram, min_len):
         eng = f_next.engine
         torch = eng.torch
         lib = eng.lib
@@ -1171,6 +1173,9 @@ class _DeviceBeam(object):
         S = len(xs)
         if _trace is not None and S != 1:
             raise ValueError('the step trace covers a group of one sentence')
+        if _trace is not None and (no_repeat_ngram or min_len):
+            raise ValueError('the step trace issues the five calls of a step without the output constraints; '
+                             'no_repeat_ngram / min_len need the one-call step')
         init_state, ctx_d, pctx_d, src_lens = f_init.group(xs)        # device tensors [S, D], [Tx, S, C], [Tx, S, A]
         Tx = int(ctx_d.shape[0])
         n = S * k
@@ -1237,6 +1242,7 @@ class _DeviceBeam(object):
         for c in (0, 1):
             m = _lib.BeamStepMany()
             m.n_src, m.src_len = S, src_len.data_ptr()
+            m.no_repeat_ngram, m.min_len = no_repeat_ngram, min_len
             a = m.beam
             a.params, a.next_w, a.ctx, a.pctx = tp_.flat.data_ptr(), next_w.data_ptr(), ctx_d.data_ptr(), pctx_d.data_ptr()
             a.Tx, a.k, a.maxlen, a.use_unk = Tx, k, maxlen, 1 if use_unk else 0
@@ -1342,28 +1348,55 @@ class _DeviceBeam(object):
         return res
 
 
-def _gen_sample_device(f_init, f_next, x, k, maxlen, use_unk, kl_factor, ctx_factor, state_factor, _trace):
+def _gen_sample_device(f_init, f_next, x, k, maxlen, use_unk, kl_factor, ctx_factor, state_factor, _trace, no_repeat_ngram=0,
+                       min_len=0):
     """one device-resident beam search (a group of one sentence) on the current stream (see _DeviceBeam)"""
-    b = _DeviceBeam(f_init, f_next, [x], k, maxlen, use_unk, kl_factor, ctx_factor, state_factor, _trace)
+    b = _DeviceBeam(f_init, f_next, [x], k, maxlen, use_unk, kl_factor, ctx_factor, state_factor, _trace,
+                    no_repeat_ngram=no_repeat_ngram, min_len=min_len)
     while b.step():
         pass
     return b.result()[0]
 
 
+def _check_constraints(no_repeat_ngram, min_len):
+    no_repeat_ngram, min_len = int(no_repeat_ngram), int(min_len)
+    if no_repeat_ngram < 0 or min_len < 0:
+        raise ValueError('no_repeat_ngram and min_len must be >= 0 (0 = off), got %d and %d' % (no_repeat_ngram, min_len))
+    return no_repeat_ngram, min_len
+
+
+def _banned_words(hyp, no_repeat_ngram, min_len):
+    """the words a live hypothesis `hyp` (its ii words, no BOS / EOS) may not take next: with N = no_repeat_ngram >= 1,
+    y[j + N - 1] for every j in [0, ii - N] with y[j : j + N - 1] == y[ii - N + 1 : ii] (N = 1: every word of hyp); EOS (0)
+    while ii < min_len.  The device step applies the same rule (beam_constrain_kernel, nats_beam_step_many)."""
+    ii, N = len(hyp), no_repeat_ngram
+    banned = set()
+    if ii < min_len:
+        banned.add(0)
+    if N >= 1 and ii >= N:
+        tail = [int(w) for w in hyp[ii - N + 1:]]
+        for j in range(ii - N + 1):
+            if [int(w) for w in hyp[j:j + N - 1]] == tail:
+                banned.add(int(hyp[j + N - 1]))
+    return sorted(banned)
+
+
 def gen_sample_many(tparams, f_init, f_next, xs, options, trng=None, k=5, maxlen=30, use_unk=False, kl_factor=0,
-                    ctx_factor=0, state_factor=0, concurrency=12, chunk=16):
+                    ctx_factor=0, state_factor=0, no_repeat_ngram=0, min_len=0, concurrency=12, chunk=16):
     """Beam search (nats.py:879-1076, stochastic=False) of a LIST of source sentences -> list of gen_sample's three lists.
     Every `chunk` consecutive sentences form one group: one masked encoder launch, then one device step advances the beams
     of all of them (S = chunk sentences x k rows per f_next; see _DeviceBeam), so the decoder and readout weights are read
     once per step for the whole group.  `concurrency` groups run interleaved, each on its own CUDA stream with its own
     workspace.  Results are those of gen_sample sentence by sentence, in order (the sentences of a group do not interact).
     Device memory per group in flight: see _DeviceBeam (3.7 GB at chunk = 16, beam 10, 100 steps, 800 source words,
-    dim 1000)."""
+    dim 1000).  no_repeat_ngram / min_len: the output constraints of gen_sample."""
+    no_repeat_ngram, min_len = _check_constraints(no_repeat_ngram, min_len)
     eng = f_next.engine
     torch = eng.torch
     if k > 32 or getattr(f_init, 'device', None) is None or os.environ.get('NATS_DEVICE_BEAM', '1') == '0':
         return [gen_sample(tparams, f_init, f_next, numpy.asarray(x).reshape(-1, 1), options, trng, k, maxlen, False, False,
-                           use_unk, kl_factor, ctx_factor, state_factor) for x in xs]
+                           use_unk, kl_factor, ctx_factor, state_factor, no_repeat_ngram=no_repeat_ngram, min_len=min_len)
+                for x in xs]
     chunk = max(1, int(chunk))
     streams = getattr(eng, '_beam_streams', None)
     if streams is None:
@@ -1379,7 +1412,7 @@ def gen_sample_many(tparams, f_init, f_next, xs, options, trng=None, k=5, maxlen
         grp = [numpy.asarray(x).reshape(-1) for x in xs[nxt:nxt + chunk]]
         streams[slot].wait_stream(main)                           # whatever the current stream queued comes first
         b = _DeviceBeam(f_init, f_next, grp, k, maxlen, use_unk, kl_factor, ctx_factor, state_factor, None, slot + 1,
-                        streams[slot])
+                        streams[slot], no_repeat_ngram, min_len)
         active[slot] = (nxt, b)
         nxt += len(grp)
         b.step()
@@ -1402,16 +1435,26 @@ def gen_sample_many(tparams, f_init, f_next, xs, options, trng=None, k=5, maxlen
 
 
 def gen_sample(tparams, f_init, f_next, x, options, trng=None, k=1, maxlen=30, stochastic=True, argmax=False,
-               use_unk=False, kl_factor=0, ctx_factor=0, state_factor=0, _scorer_factory=None, _trace=None):
+               use_unk=False, kl_factor=0, ctx_factor=0, state_factor=0, no_repeat_ngram=0, min_len=0, _scorer_factory=None,
+               _trace=None):
     """Stochastic sampling or beam search with distraction re-ranking; same arguments, return values and
     hypothesis bookkeeping as the reference (nats.py:879-1076).  Candidate costs stay un-penalised (nats.py:1004);
-    the three penalties only re-rank (nats.py:997-999)."""
+    the three penalties only re-rank (nats.py:997-999).
+
+    Output constraints of beam search (additions beyond the reference, 0 = off): no_repeat_ngram = N bans every word that
+    would repeat an N-gram of the hypothesis, min_len = L bans EOS while the hypothesis has fewer than L words (see
+    _banned_words).  A banned word gets probability 0 after the use_unk mask, so its cost is +inf."""
+    no_repeat_ngram, min_len = _check_constraints(no_repeat_ngram, min_len)
+    constrained = no_repeat_ngram > 0 or min_len > 0
+    if constrained and stochastic:
+        raise ValueError('no_repeat_ngram / min_len apply to beam search only (stochastic=False)')
     if k > 1:
         assert not stochastic, 'Beam search does not support stochastic sampling'
     if (not stochastic and _scorer_factory is None and getattr(f_next, 'next_device', None) is not None and k <= 32
             and os.environ.get('NATS_DEVICE_BEAM', '1') != '0' and numpy.ndim(x) == 2 and numpy.shape(x)[1] == 1
             and getattr(f_init, '__module__', None) == __name__ and hasattr(f_init, 'device')):
-        return _gen_sample_device(f_init, f_next, x, k, maxlen, use_unk, kl_factor, ctx_factor, state_factor, _trace)
+        return _gen_sample_device(f_init, f_next, x, k, maxlen, use_unk, kl_factor, ctx_factor, state_factor, _trace,
+                                  no_repeat_ngram, min_len)
 
     sample, sample_score, sample_dec_alphas = [], [], []
     if stochastic:
@@ -1452,7 +1495,7 @@ def gen_sample(tparams, f_init, f_next, x, options, trng=None, k=1, maxlen=30, s
         cur = (dev.get('alpha', dec_alphas), dev.get('ctx', ctxs), dev.get('state', next_state))
         n_keep = k - dead_k
         topk = getattr(f_next, 'topk', None)
-        if topk is not None and dev.get('probs') is not None and isinstance(next_p, DeviceArray) and \
+        if not constrained and topk is not None and dev.get('probs') is not None and isinstance(next_p, DeviceArray) and \
                 next_p._h is None and n_keep <= next_p.shape[1]:
             # Hypothesis scores and penalties are constant per row, so the best n_keep candidates overall are among
             # each row's n_keep most probable words: select those on the device (nats_beam_topk) instead of sorting
@@ -1476,7 +1519,13 @@ def gen_sample(tparams, f_init, f_next, x, options, trng=None, k=1, maxlen=30, s
         else:
             if not use_unk:
                 next_p[:, 1] = 1e-20
-            cand_scores = hyp_scores[:, None] - numpy.log(next_p)
+            if constrained:                                   # after the UNK mask: a banned UNK gets 0, not 1e-20
+                for r, hyp in enumerate(hyp_samples):
+                    banned = _banned_words(hyp, no_repeat_ngram, min_len)
+                    if banned:
+                        next_p[r, banned] = 0.
+            with numpy.errstate(divide='ignore'):
+                cand_scores = hyp_scores[:, None] - numpy.log(next_p)
             cand_flat = cand_scores.flatten()
             if distract and ii > 0:
                 pen = scorer.penalties(cur[0], cur[1], cur[2], live_k, kl_factor, ctx_factor, state_factor)
