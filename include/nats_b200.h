@@ -300,8 +300,8 @@ int nats_beam_step_many(nats_ctx_t* ctx, void* stream, const nats_dims_t* dims, 
 /* The library's internal GEMM engine, exposed for the parity tests: C = op(A).op(B) (+bias) (+C), row-major,
  * path 0 = exact-fp32 FFMA kernels, path 1 = wgmma 3xTF32 kernel with software loaders, path 2 = wgmma 3xTF32 kernel
  * fed by TMA (needs 16-byte aligned operands, leading dimensions multiple of 4), path 3 = the TMA-fed kernel with the
- * 128-row operand split in registers (its default for skinny products).  splitk > 1 writes splitk slabs
- * of M*ldc floats to C (the consumer kernels sum them); batch > 1 uses the given strides. */
+ * 128-row operand split in registers (its default for skinny products); any other path is an error.  splitk > 1
+ * writes splitk slabs of M*ldc floats to C (the consumer kernels sum them); batch > 1 uses the given strides. */
 int nats_debug_gemm(nats_ctx_t* ctx, void* stream, int path, int transA, int transB, int M, int N, int K,
                     const float* A, int lda, const float* B, int ldb, float* C, int ldc, const float* bias,
                     int accumulate, int splitk, int batch, int64_t strideA, int64_t strideB, int64_t strideC);

@@ -102,7 +102,6 @@ int nats_ctx_create(int device, nats_ctx_t** out) {
     tma_gemm_set_ts(getenv("NATS_TS") ? atoi(getenv("NATS_TS")) : 1);
     if (getenv("NATS_TRACE_GATES")) gates_trace(atoi(getenv("NATS_TRACE_GATES")));
     pdl_set(getenv("NATS_PDL") ? atoi(getenv("NATS_PDL")) : 1);
-    gemm_set_tensor_cores(getenv("NATS_TC") ? atoi(getenv("NATS_TC")) : 2);
     if (r != 0) { cudaFree(c->dev_scratch); delete c; return r; }
     *out = c;
     return 0;
@@ -196,11 +195,8 @@ int nats_debug_gemm(nats_ctx_t* ctx, void* stream, int path, int transA, int tra
         tma_gemm_set_ts(keep_ts);
         return r;
     }
-    const int keep = gemm_get_tensor_cores();
-    gemm_set_tensor_cores(0);
-    const int r = gemm_launch(st, &p, 1, transA != 0, transB != 0, GEMM_CFG_AUTO);
-    gemm_set_tensor_cores(keep);
-    return r;
+    NATS_REQUIRE(path == 0, "nats_debug_gemm: path must be 0, 1, 2 or 3");
+    return sgemm_launch(st, &p, 1, transA != 0, transB != 0);
 }
 
 // ------------------------------------------------------------------------------------------ profiling

@@ -261,13 +261,8 @@ __global__ void reduce_splits_kernel(const float* __restrict__ part, int nsplit,
 
 }  // namespace
 
-static int g_use_tc = 2;      // 0: FFMA, 1: wgmma with software loaders, 2: wgmma fed by TMA where possible
-void gemm_set_tensor_cores(int on) { g_use_tc = on; }
-int gemm_get_tensor_cores() { return g_use_tc; }
-
 // is this group worth a 128-row tensor-core tile?  (tiny problems stay on the FFMA kernels)
 static bool tc_eligible(const GemmProblem* probs, int count) {
-    if (!g_use_tc) return false;
     for (int i = 0; i < count; ++i) {
         const int big = probs[i].M > probs[i].N ? probs[i].M : probs[i].N;
         if (big < 64 || probs[i].K < 32) return false;
@@ -275,13 +270,18 @@ static bool tc_eligible(const GemmProblem* probs, int count) {
     return true;
 }
 
-
-int gemm_launch(cudaStream_t st, const GemmProblem* probs, int count, bool transA, bool transB, int cfg) {
+int gemm_launch(cudaStream_t st, const GemmProblem* probs, int count, bool transA, bool transB) {
     NATS_REQUIRE(count >= 1 && count <= kGemmMaxGroup, "gemm group size");
-    if (tc_eligible(probs, count)) {
-        if (g_use_tc >= 2 && tma_gemm_eligible(probs, count)) return tma_gemm_launch(st, probs, count, transA, transB);
-        return tc_gemm_launch(st, probs, count, transA, transB);
-    }
+    if (!tc_eligible(probs, count)) return sgemm_launch(st, probs, count, transA, transB);
+    if (tma_gemm_eligible(probs, count)) return tma_gemm_launch(st, probs, count, transA, transB);
+    return tc_gemm_launch(st, probs, count, transA, transB);
+}
+
+// The recurrences' per-step products take the tile here that any product of their shape takes, since of them only
+// d h1 += d ps . W_att^T could reach the 128 x 128 tile (batch >= 512, dim >= 512 and dim_att < 32) and every output
+// element sums over k in the same order whatever the tile.
+int sgemm_launch(cudaStream_t st, const GemmProblem* probs, int count, bool transA, bool transB) {
+    NATS_REQUIRE(count >= 1 && count <= kGemmMaxGroup, "gemm group size");
     GemmGroup grp;
     memset(&grp, 0, sizeof(grp));
     grp.count = count;
@@ -299,32 +299,22 @@ int gemm_launch(cudaStream_t st, const GemmProblem* probs, int count, bool trans
     grp.zstart[count] = z;
     for (int i = count; i < kGemmMaxGroup; ++i) grp.zstart[i + 1] = z;
     if (maxM == 0) return 0;
-    if (cfg == GEMM_CFG_AUTO) {
-        if (maxM <= 32) cfg = GEMM_CFG_SMALLM;
-        else if (maxM >= 512 && minN >= 512) cfg = GEMM_CFG_BIG;
-        else cfg = GEMM_CFG_MID;
-    }
-    switch (cfg) {
-        case GEMM_CFG_BIG: return launch_cfg<128, 128, 8, 8, 8>(st, grp, transA, transB);
-        case GEMM_CFG_MID: return launch_cfg<64, 64, 16, 4, 4>(st, grp, transA, transB);
-        case GEMM_CFG_SMALLM: return launch_cfg<32, 128, 16, 4, 4>(st, grp, transA, transB);
-        default: break;
-    }
-    set_error("gemm_launch: bad cfg %d", cfg);
-    return 2;
+    const SgemmTile t = sgemm_tile(maxM, minN);
+    if (t.bm == 128) return launch_cfg<128, 128, 8, 8, 8>(st, grp, transA, transB);
+    if (t.bm == 64) return launch_cfg<64, 64, 16, 4, 4>(st, grp, transA, transB);
+    return launch_cfg<32, 128, 16, 4, 4>(st, grp, transA, transB);
 }
-
-int gemm_step_cfg(int M) { return M <= 32 ? GEMM_CFG_SMALLM : GEMM_CFG_MID; }
 
 int gemm_pick_split(const nats_ctx* ctx, int M, int N, int K, int groups) {
     int tiles;
-    if (g_use_tc && (M >= 128 || N >= 128) && K >= 32) {
-        const int a = M > N ? M : N, b = M > N ? N : M;      // 128-row side / N side of the tensor-core tile
-        const int bn = b <= 32 ? 32 : b <= 64 ? 64 : b <= 112 ? 112 : 96;     // tile widths of tma_gemm_launch
-        tiles = cdiv(a, 128) * cdiv(b, bn);
-    } else {
-        const int bm = (M <= 32) ? 32 : 64, bn = (M <= 32) ? 128 : 64;
-        tiles = cdiv(N, bn) * cdiv(M, bm);
+    if ((M >= 128 || N >= 128) && K >= 32) {
+        // tc_tile(max(M, N), min(M, N)): the larger side on the 128 rows.  This differs from the launched tiling when
+        // M >= 128 and N > M (e.g. the beam-group step at S k = 160), where gemm_launch keeps M on the 128 rows.
+        const TcTile t = tc_tile(max(M, N), min(M, N));
+        tiles = cdiv(t.ma, 128) * cdiv(t.nb, t.bn);
+    } else {      // the 128 x 128 FFMA tile needs max(M, N) >= 512, so K < 32 here, where the split is 1 anyway
+        const SgemmTile t = sgemm_tile(M, N);
+        tiles = cdiv(N, t.bn) * cdiv(M, t.bm);
     }
     tiles *= (groups > 0 ? groups : 1);          // grouped launches (both encoder directions) share the machine
     int s = ctx->num_sms / (tiles > 0 ? tiles : 1);
@@ -354,21 +344,13 @@ int gemm_auto(const nats_ctx* ctx, cudaStream_t st, GemmProblem p, bool transA, 
               long long scratch_floats) {
     if (p.M == 0 || p.N == 0) return 0;
     const bool tc = tc_eligible(&p, 1);
-    int cfg = GEMM_CFG_AUTO;
     long long tiles;
     if (tc) {
-        const int a = p.M > p.N ? p.M : p.N, b = p.M > p.N ? p.N : p.M;
-        const bool swapped = p.M < 128 && p.N > p.M;
-        const int nb = swapped ? p.M : p.N, ma = swapped ? p.N : p.M;
-        (void)a; (void)b;
-        const int bn = nb <= 32 ? 32 : nb <= 64 ? 64 : nb <= 112 ? 112 : 96;
-        tiles = (long long)cdiv(ma, 128) * cdiv(nb, bn) * p.batch;
+        const TcTile t = tc_tile(p.M, p.N);
+        tiles = (long long)cdiv(t.ma, 128) * cdiv(t.nb, t.bn) * p.batch;
     } else {
-        int bm, bn;
-        if (p.M <= 32) { cfg = GEMM_CFG_SMALLM; bm = 32; bn = 128; }
-        else if (p.M >= 512 && p.N >= 512) { cfg = GEMM_CFG_BIG; bm = 128; bn = 128; }
-        else { cfg = GEMM_CFG_MID; bm = 64; bn = 64; }
-        tiles = (long long)cdiv(p.M, bm) * cdiv(p.N, bn) * p.batch;
+        const SgemmTile t = sgemm_tile(p.M, p.N);
+        tiles = (long long)cdiv(p.M, t.bm) * cdiv(p.N, t.bn) * p.batch;
     }
     int splits = 1;
     if (tc && p.batch == 1 && tiles >= ctx->num_sms && p.K >= 4096 && scratch != nullptr) {
@@ -393,11 +375,11 @@ int gemm_auto(const nats_ctx* ctx, cudaStream_t st, GemmProblem p, bool transA, 
         while (splits > 1 && (long long)splits * p.M * p.N > scratch_floats) --splits;
         if (splits < 1) splits = 1;
     }
-    if (splits == 1) return gemm_launch(st, &p, 1, transA, transB, cfg);
+    if (splits == 1) return gemm_launch(st, &p, 1, transA, transB);
     GemmProblem q = p;
     q.C = scratch; q.ldc = p.N; q.bias = nullptr; q.accumulate = 0;
     gemm_set_split(q, splits, (long long)p.M * p.N);
-    NATS_TRY(gemm_launch(st, &q, 1, transA, transB, cfg));
+    NATS_TRY(gemm_launch(st, &q, 1, transA, transB));
     return reduce_splits(st, scratch, splits, (long long)p.M * p.N, p.M, p.N, p.N, p.C, p.ldc, p.bias, p.accumulate);
 }
 

@@ -5,7 +5,9 @@
 // grouped (up to 4 problems per launch: e.g. both encoder directions), batched (strided), split-K
 // (each split writes its own partial slab, summed by the consumer kernel => deterministic, no atomics).
 //
-// Two engines: exact-fp32 FFMA tiles (gemm.cu) and fp32-grade 3xTF32 products on the tensor cores (tc_gemm.cu, wgmma).
+// Three engines, chosen by gemm_launch from the problems alone: exact-fp32 FFMA tiles (gemm.cu) for products below 64
+// rows or 32 deep, and fp32-grade 3xTF32 products on the tensor cores (wgmma): fed by TMA where the operands allow it
+// (tma_gemm.cu), else by software loaders (tc_gemm.cu).
 #pragma once
 #include "common.cuh"
 
@@ -36,7 +38,27 @@ struct GemmGroup {
     int count;
 };
 
-enum GemmCfg { GEMM_CFG_AUTO = 0, GEMM_CFG_BIG = 1, GEMM_CFG_MID = 2, GEMM_CFG_SMALLM = 3 };
+// Tile of the FFMA engine for a group whose largest M is maxM and smallest N is minN.
+struct SgemmTile { int bm, bn; };
+inline SgemmTile sgemm_tile(int maxM, int minN) {
+    if (maxM <= 32) return {32, 128};
+    if (maxM >= 512 && minN >= 512) return {128, 128};
+    return {64, 64};
+}
+
+// Operand roles and N tile of the tensor-core engines for a group whose largest problem is maxM x maxN.  The larger
+// dimension goes on the 128-row side unless M already fills it ("swapped": skinny products put the weights on the
+// 128-row side, the batch on the N side, and store transposed).  ma / nb: the 128-row / N extents; bn: the TMA
+// engine's tile width (the software-loader engine caps it at 64).
+struct TcTile { bool swapped; int ma, nb, bn; };
+inline TcTile tc_tile(int maxM, int maxN) {
+    TcTile t;
+    t.swapped = maxM < 128 && maxN > maxM;
+    t.ma = t.swapped ? maxN : maxM;
+    t.nb = t.swapped ? maxM : maxN;
+    t.bn = t.nb <= 32 ? 32 : t.nb <= 64 ? 64 : t.nb <= 112 ? 112 : 96;
+    return t;
+}
 
 inline GemmProblem gemm_problem(const float* A, int lda, const float* B, int ldb, float* C, int ldc,
                                 int M, int N, int K) {
@@ -57,22 +79,26 @@ inline void gemm_set_split(GemmProblem& p, int splits, long long strideP) {
     p.splitk = splits;
     p.strideP = strideP;
 }
+// K range per split of the tensor-core engines: the split's chunk rounded up to whole 32-deep k-blocks
+inline int tc_kchunk(const GemmProblem& q) {
+    const int chunk = q.splitk > 1 ? cdiv(q.K, q.splitk) : q.kchunk;
+    return chunk > 0 ? ((chunk + 31) / 32) * 32 : 32;
+}
 
-// tensor-core path (tc_gemm.cu): same contract as gemm_launch, 3xTF32 on wgmma
+// The engines gemm_launch picks from, also called directly by nats_debug_gemm.  FFMA (gemm.cu): any shape.
+int sgemm_launch(cudaStream_t st, const GemmProblem* probs, int count, bool transA, bool transB);
+// tensor-core path (tc_gemm.cu): 3xTF32 on wgmma
 int tc_gemm_launch(cudaStream_t st, const GemmProblem* probs, int count, bool transA, bool transB);
 int tc_gemm_setup();
 // TMA-fed variant (tma_gemm.cu): needs 16-byte aligned operands with leading dimensions multiple of 4
 int tma_gemm_launch(cudaStream_t st, const GemmProblem* probs, int count, bool transA, bool transB);
 bool tma_gemm_eligible(const GemmProblem* probs, int count);
 int tma_gemm_setup();
-void gemm_set_tensor_cores(int on);     // 2 (default): tensor cores, TMA-fed where possible; 1: software loaders only; 0: FFMA
-int gemm_get_tensor_cores();
 
-// Low-level launch: all problems share transposition flags and tile configuration.
-int gemm_launch(cudaStream_t st, const GemmProblem* probs, int count, bool transA, bool transB, int cfg);
+// Low-level launch: all problems share transposition flags; the engine and its tile are chosen from the problems.
+int gemm_launch(cudaStream_t st, const GemmProblem* probs, int count, bool transA, bool transB);
 
-// Tile configuration and number of K-splits that fill the machine for a skinny (M = batch) weight-streaming product.
-int gemm_step_cfg(int M);
+// Number of K-splits that fill the machine for a skinny (M = batch) weight-streaming product.
 int gemm_pick_split(const nats_ctx* ctx, int M, int N, int K, int groups = 1);
 
 // Convenience: single problem, picks the tile configuration; if the problem would launch too few CTAs and K

@@ -47,7 +47,6 @@ int train_decoder_bwd(const nats_ctx* ctx, cudaStream_t st, const nats_dims_t& d
     const ParamOff o = param_offsets(d);
     const int W = d.dim_word, D = d.dim, A = d.dim_att, V = d.n_words, C = 2 * D, D3 = 3 * D;
     const long long XB = (long long)Tx * B, YB = (long long)Ty * B;
-    const int cfg = gemm_step_cfg(B);
     const int SA = gemm_pick_split(ctx, B, D, D3);    // d h1   <- dG1 . U1cat^T      (slabs in part_b)
     const int SB = gemm_pick_split(ctx, B, C, D3);    // d ctx  <- dG1x . W1cat^T     (slabs in part_a)
     const int S4 = gemm_pick_split(ctx, B, D, D3);    // d h_   <- dG2 . Ucat^T       (slabs in part_c)
@@ -83,7 +82,7 @@ int train_decoder_bwd(const nats_ctx* ctx, cudaStream_t st, const nats_dims_t& d
             gemm_set_split(q[0], SA, spD);
             q[1] = gemm_problem(w.dG1x + r3, D3, params + o.W1cat, D3, w.part_a, C, B, C, D3);
             gemm_set_split(q[1], SB, spC);
-            NATS_TRY(gemm_launch(st, q, 2, false, true, cfg));
+            NATS_TRY(gemm_launch(st, q, 2, false, true));
         }
         {   // distraction + attention backward (nats.py:527-546, 569-570)
             AttBwd a;
@@ -110,7 +109,7 @@ int train_decoder_bwd(const nats_ctx* ctx, cudaStream_t st, const nats_dims_t& d
         }
         {   // d h1 += d ps . W_att^T  (nats.py:527)
             GemmProblem q = gemm_problem(w.dps + rA, A, params + o.W_att, A, w.part_d, D, B, D, A);
-            NATS_TRY(gemm_launch(st, &q, 1, false, true, cfg));
+            NATS_TRY(gemm_launch(st, &q, 1, false, true));
         }
         {   // GRU_2 backward (nats.py:505-518)
             GateBwd g;
@@ -127,7 +126,7 @@ int train_decoder_bwd(const nats_ctx* ctx, cudaStream_t st, const nats_dims_t& d
         {   // d h_{t-1} through the GRU_2 recurrent product
             GemmProblem q = gemm_problem(w.dG2 + r3, D3, params + o.dec.Ucat, D3, w.part_c, D, B, D, D3);
             gemm_set_split(q, S4, spD);
-            NATS_TRY(gemm_launch(st, &q, 1, false, true, cfg));
+            NATS_TRY(gemm_launch(st, &q, 1, false, true));
         }
     }
     // d init_state -> pre-activation of ff_state (nats.py:723-724)
@@ -161,7 +160,7 @@ int train_decoder_bwd(const nats_ctx* ctx, cudaStream_t st, const nats_dims_t& d
     {   // dcc[:, b, :] += alpha_b^T [Tx,Ty] . dcraw_b [Ty,C]   -- one batched product instead of Ty rank-1 updates
         GemmProblem p = gemm_problem(w.d_alpha, B * Tx, w.dcraw, B * C, w.dcc, B * C, Tx, C, Ty);
         p.batch = B; p.strideA = Tx; p.strideB = C; p.strideC = C; p.accumulate = 1;
-        NATS_TRY(gemm_launch(st, &p, 1, true, false, GEMM_CFG_AUTO));
+        NATS_TRY(gemm_launch(st, &p, 1, true, false));
     }
     // ---- d target embedding (nats.py:487-491, 730-734)
     {
@@ -185,7 +184,6 @@ int train_encoder_bwd(const nats_ctx* ctx, cudaStream_t st, const nats_dims_t& d
     const ParamOff o = param_offsets(d);
     const int W = d.dim_word, D = d.dim, V = d.n_words, C = 2 * D, D3 = 3 * D;
     const long long XB = (long long)Tx * B;
-    const int cfg = gemm_step_cfg(B);
     const int S = gemm_pick_split(ctx, B, D, D3, 2);
     const long long strideP = 2LL * B * D;
     const bool persistent = enc_tc_eligible(ctx, B, D, 1);
@@ -235,7 +233,7 @@ int train_encoder_bwd(const nats_ctx* ctx, cudaStream_t st, const nats_dims_t& d
                                       w.part_a + (long long)dir * B * D, D, B, D, D3);
                 gemm_set_split(q[dir], S, strideP);
             }
-            NATS_TRY(gemm_launch(st, q, 2, false, true, cfg));
+            NATS_TRY(gemm_launch(st, q, 2, false, true));
         }
     }
     if (Tx > 1) {

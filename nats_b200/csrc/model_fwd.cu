@@ -22,11 +22,10 @@ int encoder_forward(const nats_ctx* ctx, cudaStream_t st, const nats_dims_t& d, 
             pr[dir] = gemm_problem(e.emb_x, W, params + o.enc[dir].Wcat, D3, e.xproj[dir], D3, (int)XB, D3, W);
             pr[dir].bias = params + o.enc[dir].bcat;
         }
-        NATS_TRY(gemm_launch(st, pr, 2, false, false, GEMM_CFG_AUTO));
+        NATS_TRY(gemm_launch(st, pr, 2, false, false));
     }
     NATS_CUDA_OK(memset_async(st, e.ctxsum, 0, (size_t)n * C * sizeof(float)));
     const int S = gemm_pick_split(ctx, n, D3, D, 2);
-    const int cfg = gemm_step_cfg(n);
     const long long strideP = 2LL * n * D3;
     if (enc_tc_eligible(ctx, n, D, 0) && e.enc_scratch != nullptr) {
         // the whole recurrence of both directions in ONE persistent weight-stationary wgmma launch (enc_tc.cu)
@@ -52,7 +51,7 @@ int encoder_forward(const nats_ctx* ctx, cudaStream_t st, const nats_dims_t& d, 
                                     e.part_a + (long long)n * D3, D3, n, D3, D);
                 gemm_set_split(q[0], S, strideP);
                 gemm_set_split(q[1], S, strideP);
-                NATS_TRY(gemm_launch(st, q, 2, false, false, cfg));
+                NATS_TRY(gemm_launch(st, q, 2, false, false));
             }
             GateFwd g[2];
             memset(g, 0, sizeof(g));
@@ -96,14 +95,13 @@ int decoder_step_forward(const nats_ctx* ctx, cudaStream_t st, const nats_dims_t
                          const DecStep& s) {
     const ParamOff o = param_offsets(d);
     const int D = d.dim, A = d.dim_att, C = 2 * D, D3 = 3 * D, n = s.n;
-    const int cfg = gemm_step_cfg(n);
     const int S1 = gemm_pick_split(ctx, n, D3, D);
     const int S2 = gemm_pick_split(ctx, n, D3, C);
     const long long sp3 = (long long)n * D3;
     {   // GRU_2 recurrent product (nats.py:505, 512)
         GemmProblem q = gemm_problem(s.h_prev, D, params + o.dec.Ucat, D3, s.part_b, D3, n, D3, D);
         gemm_set_split(q, S1, sp3);
-        NATS_TRY(gemm_launch(st, &q, 1, false, false, cfg));
+        NATS_TRY(gemm_launch(st, &q, 1, false, false));
         GateFwd g;
         memset(&g, 0, sizeof(g));
         g.part = s.part_b; g.nsplit = S1; g.part_stride = sp3;
@@ -120,7 +118,7 @@ int decoder_step_forward(const nats_ctx* ctx, cudaStream_t st, const nats_dims_t
         gemm_set_split(q[0], S1, sp3);
         q[1] = gemm_problem(s.h1, D, params + o.W_att, A, s.part_d, A, n, A, D);
         gemm_set_split(q[1], S1, (long long)n * A);
-        NATS_TRY(gemm_launch(st, q, 2, false, false, cfg));
+        NATS_TRY(gemm_launch(st, q, 2, false, false));
     }
     {
         AttFwd a;
@@ -143,7 +141,7 @@ int decoder_step_forward(const nats_ctx* ctx, cudaStream_t st, const nats_dims_t
     {   // GRU_1 (nats.py:551-565)
         GemmProblem q = gemm_problem(s.ctx_out, C, params + o.W1cat, D3, s.part_a, D3, n, D3, C);
         gemm_set_split(q, S2, sp3);
-        NATS_TRY(gemm_launch(st, &q, 1, false, false, cfg));
+        NATS_TRY(gemm_launch(st, &q, 1, false, false));
         GateFwd g;
         memset(&g, 0, sizeof(g));
         g.part = s.part_c; g.nsplit = S1; g.part_stride = sp3;

@@ -231,10 +231,8 @@ int tc_gemm_launch(cudaStream_t st, const GemmProblem* probs, int count, bool tr
     int z = 0, maxM = 0, maxN = 0;
     for (int i = 0; i < count; ++i) { maxM = max(maxM, probs[i].M); maxN = max(maxN, probs[i].N); }
     if (maxM == 0 || maxN == 0) return 0;
-    // operand roles: the 128-row side should be the larger dimension
-    const bool swapped = maxM < 128 && maxN > maxM;
-    const int nb_dim = swapped ? maxM : maxN;
-    const int BN = nb_dim <= 32 ? 32 : 64;
+    const TcTile tile = tc_tile(maxM, maxN);
+    const bool swapped = tile.swapped;
     for (int i = 0; i < count; ++i) {
         const GemmProblem& q = probs[i];
         NATS_REQUIRE(q.splitk >= 1 && q.batch >= 1 && (q.splitk == 1 || !q.accumulate), "tc gemm split/batch");
@@ -253,19 +251,14 @@ int tc_gemm_launch(cudaStream_t st, const GemmProblem* probs, int count, bool tr
         }
         t.C = q.C; t.bias = q.bias; t.K = q.K; t.batch = q.batch; t.sC = q.strideC;
         t.splitk = q.splitk;
-        t.kchunk = ((q.kchunk + 31) / 32) * 32;
-        if (q.splitk > 1) {
-            int chunk = (q.K + q.splitk - 1) / q.splitk;
-            t.kchunk = ((chunk + 31) / 32) * 32;
-        }
-        if (t.kchunk <= 0) t.kchunk = 32;
+        t.kchunk = tc_kchunk(q);
         t.strideP = q.strideP; t.accumulate = q.accumulate;
         grp.zstart[i] = z;
         z += q.batch * q.splitk;
     }
     grp.zstart[count] = z;
     for (int i = count; i < kTcMaxGroup; ++i) grp.zstart[i + 1] = z;
-    return BN == 32 ? tc_launch<32>(st, grp, true) : tc_launch<64>(st, grp, nb_dim <= 64);
+    return tile.bn == 32 ? tc_launch<32>(st, grp, true) : tc_launch<64>(st, grp, tile.nb <= 64);
 }
 
 }  // namespace nats

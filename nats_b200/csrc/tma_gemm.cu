@@ -667,10 +667,9 @@ int tma_gemm_launch(cudaStream_t st, const GemmProblem* probs, int count, bool t
     grp.count = count;
     int maxM = 0, maxN = 0;
     for (int i = 0; i < count; ++i) { maxM = max(maxM, probs[i].M); maxN = max(maxN, probs[i].N); }
-    const bool swapped = maxM < 128 && maxN > maxM;
-    const int nb_dim = swapped ? maxM : maxN;
-    const bool skinny = nb_dim <= 64;
-    const int BN = nb_dim <= 32 ? 32 : nb_dim <= 64 ? 64 : nb_dim <= 112 ? 112 : 96;
+    const TcTile tile = tc_tile(maxM, maxN);
+    const bool swapped = tile.swapped, skinny = tile.nb <= 64;
+    const int BN = tile.bn;
     // op(A)(m,k): transA ? m contiguous : k contiguous.  op(B)(k,n): transB ? k contiguous : n contiguous.
     const bool opa_mn = transA, opb_mn = !transB;
     const bool a_mn = swapped ? opb_mn : opa_mn;      // the 128-row side operand
@@ -699,9 +698,7 @@ int tma_gemm_launch(cudaStream_t st, const GemmProblem* probs, int count, bool t
         else { t.c_rs = 1; t.c_cs = q.ldc; t.bias_on_a = 1; }
         t.C = q.C; t.bias = q.bias; t.K = q.K; t.batch = q.batch; t.sC = q.strideC;
         t.splitk = q.splitk;
-        t.kchunk = ((q.kchunk + 31) / 32) * 32;
-        if (q.splitk > 1) t.kchunk = ((cdiv(q.K, q.splitk) + 31) / 32) * 32;
-        if (t.kchunk <= 0) t.kchunk = 32;
+        t.kchunk = tc_kchunk(q);
         t.strideP = q.strideP; t.accumulate = q.accumulate;
         grp.zstart[i] = z;
         grp.istart[i] = items;

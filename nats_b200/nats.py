@@ -17,6 +17,7 @@ Pure-host helpers (init_params, prepare_data, load_params, the beam bookkeeping 
 from collections import OrderedDict
 import copy
 import ctypes
+import gc
 import logging
 import os
 import pickle as pkl
@@ -535,8 +536,17 @@ class ModelGraph(object):
         if self.use_graphs and p.uses >= 1:
             torch.cuda.synchronize(self.engine.device)
             g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g):
-                body()
+            # A dead reference cycle may hold a CUDA graph or other CUDA objects; their finalizers must not run while the
+            # stream is capturing (in any thread), or the capture is invalidated.  So: collect before, no collector during.
+            gc.collect()
+            gc_on = gc.isenabled()
+            gc.disable()
+            try:
+                with torch.cuda.graph(g):
+                    body()
+            finally:
+                if gc_on:
+                    gc.enable()
             setattr(p, attr, g)
             g.replay()
             return

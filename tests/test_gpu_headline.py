@@ -195,8 +195,6 @@ SWITCHES = [
     {'NATS_ENC_TC': '0'},                 # per-step encoder path instead of the persistent tensor-core kernel
     {'NATS_ENC_TC': '2'},                 # persistent forward + per-step backward
     {'NATS_ENC_TC': '3'},                 # per-step forward + persistent backward
-    {'NATS_TC': '0'},                     # exact-fp32 FFMA products everywhere
-    {'NATS_TC': '1'},                     # wgmma with software loaders (no TMA)
     {'NATS_TS': '0'},                     # skinny products split in shared memory instead of registers
     {'NATS_PDL': '0'},                    # no programmatic dependent launch
     # beam-search kernels: one CTA per row / per (row, slice) and library GEMMs instead of the 8-CTA cluster kernels
