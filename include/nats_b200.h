@@ -296,6 +296,59 @@ typedef struct nats_beam_step_many {
 } nats_beam_step_many_t;
 int nats_beam_step_many(nats_ctx_t* ctx, void* stream, const nats_dims_t* dims, const nats_beam_step_many_t* a, int step);
 
+/* Filtered sampling (an addition beyond the reference): one step draws the next word of n = S*R independent rows, R
+ * samples of each of S sources, in one call: nats_sampler_next on all n rows (row r = s*R + j attends to source s, as in
+ * nats_beam_step_many; no multinomial draw) -> the bans when a constraint is on -> the filtered draw -> the bookkeeping.
+ * Rows never branch, so nothing is gathered: the caller swaps the state / acc_ctx / acc_alpha ping-pong buffers (`*_out` of
+ * step ii is `*_in` of step ii + 1).  Layouts (n = S*R):
+ *   ctx [Tx, S, 2*dim], pctx [Tx, S, dim_att], src_len [S] (device int32): as for nats_beam_step_many;
+ *   ws: nats_sampler_workspace_bytes(dims, Tx, n); next_w [n] (int64; -1 = BOS before step 0; receives the drawn words);
+ *   state_* [n, dim] (state_in of step 0: each source's init_state on its R rows), acc_ctx_* [n, 2*dim] and acc_alpha_*
+ *     [n, Tx] (zeros at step 0), probs [n, n_words], alphaT [n, Tx], ctxs [n, 2*dim]: f_next's outputs;
+ *   pick [n] (int32 scratch), done [n] (int32, zeros at step 0), tokens [n, maxlen] (int32), cost [n] (float, zeros at
+ *     step 0), out_len [n] (int32, maxlen at step 0), out_alpha [n, maxlen, Tx];
+ *   counters [8 + S] (int32, zeros at step 0): [0] finished rows of the group, [1] used by the kernel, [8 + s] finished
+ *     rows of source s; host_counters (NULL = off): page-locked host memory, int32[8]; [0] receives counters[0], so the
+ *     host polls one flag for the whole group.
+ * Row r is the global row q = row_base + r (row_base = (index of the group's first source) * R), and at step ii a row that
+ * is not done does:
+ *   1. p = its f_next probabilities.  A word is banned when it is UNK (1) and use_unk == 0, EOS (0) while ii < min_len, or
+ *      it would complete an N-gram the row already contains (no_repeat_ngram = N, the rule of nats_beam_step_many).
+ *   2. Banned words get weight 0, every other word w_v = (p_v / p_max)^(1/T), p_max the largest admissible p (T = 1:
+ *      w = p exactly).
+ *   3. Sorted order: w descending, ties by lower index first.  top_k = K >= 1 keeps the first K words with w > 0; top_p =
+ *      P < 1 then keeps the shortest prefix of those whose weight sum is >= P x their total.  (The kernel sums these
+ *      weights in 2^-40 fixed point of the largest weight, exact and independent of order: below n_words * 2^-40 of it.)
+ *   4. u = uniform01(seed, ii, q) (the counter-based splitmix64 uniform of nats_sampler_next), Z = the kept total: the word
+ *      is the smallest kept v with u*Z < sum of the kept w up to v in vocabulary order (rounding: the last kept word).  A
+ *      word of weight 0 is never drawn.  When (p_v / p_max)^(1/T) underflows to 0 in float32 (small T), fewer words may
+ *      carry weight than top_k asks for: then all of them are kept.  With no admissible word the row ends with word 0.
+ *   5. tokens[q][ii] = v, cost[q] += -log p_v (the unfiltered f_next probability, as beam search's stored cost),
+ *      out_alpha[q][ii] = its attention row; word 0 ends the row with out_len[q] = ii + 1 (EOS included).  A row forced to
+ *      end also pays -log p_0 of its unfiltered probability: the EOS and UNK bans act in the draw, probs keeps f_next's
+ *      values except the n-gram bans' zeros (which never hit EOS).
+ * A row's draws depend only on (seed, step, q) and its own words: not on the group, its size or the other rows.  Every
+ * reduction has a fixed order, so a repeated call gives the same bits.
+ * Errors: temperature <= 0 or NaN, top_k < 0, top_p outside (0, 1] or NaN, R < 1, S < 1, S*R > 65535, negative
+ * constraints, a constraint on with maxlen > 12288, NULL buffers. */
+typedef struct nats_sample_step_many {
+    const float* params;                 /* flat parameter buffer */
+    int64_t* next_w;                     /* [n] */
+    const float* ctx; const float* pctx; /* [Tx, S, 2*dim], [Tx, S, dim_att] */
+    const int32_t* src_len;              /* [S] device */
+    int32_t Tx, n_src, n_samples, maxlen; /* Tx = longest source, S, R, steps */
+    int32_t use_unk, top_k, no_repeat_ngram, min_len;
+    float temperature, top_p;
+    uint64_t seed, row_base;
+    void* ws; int64_t ws_bytes;
+    const float* state_in; const float* acc_ctx_in; const float* acc_alpha_in;
+    float* state_out; float* acc_ctx_out; float* acc_alpha_out;
+    float* probs; float* alphaT; float* ctxs;
+    int32_t* pick; int32_t* done; int32_t* tokens; float* cost; int32_t* out_len; float* out_alpha;
+    int32_t* counters; int32_t* host_counters;
+} nats_sample_step_many_t;
+int nats_sample_step_many(nats_ctx_t* ctx, void* stream, const nats_dims_t* dims, const nats_sample_step_many_t* a, int step);
+
 /* ---------------------------------------------------------------- diagnostics ------------------- */
 /* The library's internal GEMM engine, exposed for the parity tests: C = op(A).op(B) (+bias) (+C), row-major,
  * path 0 = exact-fp32 FFMA kernels, path 1 = wgmma 3xTF32 kernel with software loaders, path 2 = wgmma 3xTF32 kernel

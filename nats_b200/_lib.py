@@ -43,6 +43,18 @@ class BeamStepMany(Structure):
     """nats_beam_step_many_t of include/nats_b200.h: a group of n_src sentences x k rows, with the output constraints"""
     _fields_ = [('beam', BeamStep), ('n_src', c_int32), ('src_len', _P), ('no_repeat_ngram', c_int32), ('min_len', c_int32)]
 
+
+class SampleStepMany(Structure):
+    """nats_sample_step_many_t of include/nats_b200.h, field for field: filtered sampling of n_src sources x n_samples rows"""
+    _fields_ = ([(n, _P) for n in ('params', 'next_w', 'ctx', 'pctx', 'src_len')] +
+                [(n, c_int32) for n in ('Tx', 'n_src', 'n_samples', 'maxlen', 'use_unk', 'top_k', 'no_repeat_ngram',
+                                        'min_len')] +
+                [('temperature', c_float), ('top_p', c_float), ('seed', c_uint64), ('row_base', c_uint64),
+                 ('ws', _P), ('ws_bytes', c_int64)] +
+                [(n, _P) for n in ('state_in', 'acc_ctx_in', 'acc_alpha_in', 'state_out', 'acc_ctx_out', 'acc_alpha_out',
+                                   'probs', 'alphaT', 'ctxs', 'pick', 'done', 'tokens', 'cost', 'out_len', 'out_alpha',
+                                   'counters', 'host_counters')])
+
 # name -> (restype, argtypes); mirrors include/nats_b200.h one to one (checked by tests/test_abi.py)
 SIGNATURES = {
     'nats_last_error': (c_char_p, []),
@@ -87,6 +99,7 @@ SIGNATURES = {
     'nats_beam_advance': (c_int, [c_void_p, _P] + [_P] * 3 + [c_int] * 6 + [_P] * 16),
     'nats_beam_step': (c_int, [c_void_p, _P, POINTER(Dims), POINTER(BeamStep), c_int]),
     'nats_beam_step_many': (c_int, [c_void_p, _P, POINTER(Dims), POINTER(BeamStepMany), c_int]),
+    'nats_sample_step_many': (c_int, [c_void_p, _P, POINTER(Dims), POINTER(SampleStepMany), c_int]),
     'nats_debug_gemm': (c_int, [c_void_p, _P, c_int, c_int, c_int, c_int, c_int, c_int, _P, c_int, _P, c_int, _P, c_int,
                                 _P, c_int, c_int, c_int, c_int64, c_int64, c_int64]),
     'nats_profile_enable': (c_int, [c_void_p, c_int]),

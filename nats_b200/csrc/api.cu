@@ -31,7 +31,7 @@ const char* kNames[K_COUNT] = {
     "gemm_mid_tt", "gemm_smallm_nn", "gemm_smallm_nt", "gemm_smallm_tn", "gemm_smallm_tt", "gru_gates_fwd",
     "gru_gates_bwd", "att_scores", "att_context", "att_bwd_ctx", "att_bwd_dalpha", "att_bwd_softmax", "nll_rows",
     "dlogits", "softmax_sample", "colsum", "reduce_splits", "embedding", "elementwise", "optimizer", "beam",
-    "memset", "tc_gemm_3xtf32", "tc_gemm_3xtf32_skinny", "enc_tc_fwd", "enc_tc_bwd"};
+    "memset", "tc_gemm_3xtf32", "tc_gemm_3xtf32_skinny", "enc_tc_fwd", "enc_tc_bwd", "sample"};
 }  // namespace
 const char* kclass_name(int cls) { return (cls >= 0 && cls < K_COUNT) ? kNames[cls] : "?"; }
 bool prof_enabled() { return g_prof.on; }
@@ -75,7 +75,7 @@ struct ViewDef { const char* name; int64_t off; int rows, cols, ld, ndim; };
 extern "C" {
 
 const char* nats_last_error(void) { return g_err; }
-int nats_version(void) { return 102; }
+int nats_version(void) { return 103; }
 
 int nats_ctx_create(int device, nats_ctx_t** out) {
     NATS_REQUIRE(out != nullptr, "out");
@@ -627,6 +627,50 @@ int nats_beam_step_many(nats_ctx_t* ctx, void* stream, const nats_dims_t* dims, 
                  "no_repeat_ngram / min_len need maxlen <= 12288");
     return beam_step_group(ctx, reinterpret_cast<cudaStream_t>(stream), dims, &a->beam, a->n_src, a->src_len,
                            a->no_repeat_ngram, a->min_len, step);
+}
+
+}  // extern "C"
+
+namespace {
+
+// One sampling step of a group of n_src sources x R rows (the sibling of beam_step_group): f_next on all rows, each
+// attending to its own source, the bans when a constraint is on, the filtered draw, the bookkeeping.
+int sample_step_group(nats_ctx_t* ctx, cudaStream_t st, const nats_dims_t* dims, const nats_sample_step_many_t* a, int step) {
+    NATS_REQUIRE(ctx && dims && a, "null argument");
+    NATS_REQUIRE(a->temperature > 0.f, "temperature must be > 0");
+    NATS_REQUIRE(a->top_k >= 0, "top_k must be >= 0 (0 = off)");
+    NATS_REQUIRE(a->top_p > 0.f && a->top_p <= 1.f, "top_p must be in (0, 1] (1 = off)");
+    NATS_REQUIRE(a->n_samples >= 1, "n_samples must be >= 1");
+    NATS_REQUIRE(a->n_src >= 1 && (long long)a->n_src * a->n_samples <= 65535, "sampling group size (1 <= S*R <= 65535)");
+    NATS_REQUIRE(a->no_repeat_ngram >= 0 && a->min_len >= 0, "no_repeat_ngram and min_len must be >= 0");
+    NATS_REQUIRE((a->no_repeat_ngram == 0 && a->min_len == 0) || a->maxlen <= kBeamConstrainMaxLen,
+                 "no_repeat_ngram / min_len need maxlen <= 12288");
+    NATS_REQUIRE(a->Tx >= 1 && a->maxlen >= 1 && step >= 0 && step < a->maxlen, "sampling step shape");
+    NATS_REQUIRE(a->src_len && a->next_w && a->probs && a->pick && a->done && a->tokens && a->cost && a->out_len &&
+                     a->out_alpha && a->counters, "null argument");
+    NATS_TRY(check_dims(dims));
+    const int D = dims->dim, C = 2 * D, A = dims->dim_att, V = dims->n_words, S = a->n_src, R = a->n_samples, n = S * R;
+    const int64_t cbs = S == 1 ? 0 : C, pbs = S == 1 ? 0 : A;
+    NATS_TRY(sampler_next(ctx, reinterpret_cast<void*>(st), dims, a->params, a->next_w, a->ctx, (int64_t)S * C, cbs, a->pctx,
+                          (int64_t)S * A, pbs, R, a->src_len, a->state_in, a->acc_ctx_in, a->acc_alpha_in, a->Tx, n, 0, 0, a->ws,
+                          a->ws_bytes, a->probs, nullptr, a->state_out, a->alphaT, a->ctxs, a->acc_ctx_out, a->acc_alpha_out));
+    // n-gram bans zero entries of probs; a row's words never include EOS, so probs[.][0] keeps its f_next value, and the
+    // EOS ban of min_len (like the UNK ban) is applied inside the draw: a row forced to end pays -log of that value
+    if (a->no_repeat_ngram > 0)
+        NATS_TRY(sample_constrain(st, a->probs, V, a->tokens, a->maxlen, step, n, a->done, a->no_repeat_ngram, 0));
+    NATS_TRY(sample_filter(st, a->probs, n, V, a->done, a->use_unk ? 0 : 1, step < a->min_len ? 1 : 0, a->temperature,
+                           a->top_k, a->top_p, a->seed, step, a->row_base, a->pick));
+    NATS_TRY(sample_advance(st, a->pick, a->probs, V, a->alphaT, a->Tx, S, R, a->maxlen, step, a->done, a->tokens, a->cost,
+                            a->out_len, a->out_alpha, reinterpret_cast<long long*>(a->next_w), a->counters, a->host_counters));
+    return 0;
+}
+
+}  // namespace
+
+extern "C" {
+
+int nats_sample_step_many(nats_ctx_t* ctx, void* stream, const nats_dims_t* dims, const nats_sample_step_many_t* a, int step) {
+    return sample_step_group(ctx, reinterpret_cast<cudaStream_t>(stream), dims, a, step);
 }
 
 

@@ -174,6 +174,11 @@ int dlogits_inplace(cudaStream_t st, float* logits, int rows, int V, const int64
 // probs[r,:] = softmax(logits[r,:]); sample[r] ~ multinomial(probs[r,:]) (counter-based RNG)
 int softmax_sample_rows(cudaStream_t st, const float* logits, int rows, int V, float* probs, int64_t* sample,
                         uint64_t seed, uint64_t step);
+// filtered sampling of one word per row that is not done (row_done[r] != 0 skips row r; NULL = every row): UNK banned
+// when mask_unk, EOS when ban_eos (probs itself is not changed), temperature, top-k (0 = off), top-p (1 = off), draw with
+// uniform01(seed, step, row_base + r); pick [rows]; see ops_readout.cu and nats_sample_step_many in include/nats_b200.h
+int sample_filter(cudaStream_t st, const float* probs, int rows, int V, const int32_t* row_done, int mask_unk, int ban_eos,
+                  float temperature, int top_k, float top_p, uint64_t seed, int step, uint64_t row_base, int32_t* pick);
 
 // ------------------------------------------------------------------ optimiser (nats.py:1106-1206, 1326-1353)
 int grad_clip(const nats_ctx* ctx, cudaStream_t st, long long n, const float* params, float* grads, float decay_c,
@@ -201,6 +206,15 @@ int beam_reorder_append(cudaStream_t st, const float* src, float* dst, const flo
 constexpr int kBeamConstrainMaxLen = 12288;   // a row's history is staged in (at most 48 KB of) shared memory
 int beam_constrain(cudaStream_t st, float* probs, int V, const int32_t* tokens, int maxlen, int step, int n_src, int k,
                    const int32_t* counters, int no_repeat, int min_len, int mask_unk);
+// the same bans on the n rows of a sampling group (tokens [n, maxlen]: each row's own words; rows with row_done[r] != 0
+// are skipped); the sampling step passes min_len = 0 and leaves the EOS and UNK bans to sample_filter
+int sample_constrain(cudaStream_t st, float* probs, int V, const int32_t* tokens, int maxlen, int step, int n,
+                     const int32_t* row_done, int no_repeat, int min_len);
+// bookkeeping of one sampling step for a group of n_src sources x R rows (pick -> tokens, cost, lengths, attention,
+// next_w, the group's count of finished rows): see ops_beam.cu
+int sample_advance(cudaStream_t st, const int32_t* pick, const float* probs, int V, const float* alphaT, int Tx, int n_src,
+                   int R, int maxlen, int step, int32_t* done, int32_t* tokens, float* cost, int32_t* out_len, float* out_alpha,
+                   long long* next_w, int32_t* counters, int32_t* host_counters);
 // device-resident bookkeeping of one beam step (nats.py:976-1066) for a group of n_src sentences x k rows: see ops_beam.cu
 int beam_select(cudaStream_t st, const float* top_p, const int32_t* top_i, const float* pen, int n_src, int k, int maxlen,
                 int step, int32_t* counters, float* scores, int32_t* tokens, int32_t* parents, long long* next_w,

@@ -312,12 +312,14 @@ __global__ void __launch_bounds__(256) beam_advance_kernel(const __grid_constant
 // no_repeat = N >= 1, for every start j in [0, step - N] whose N-1 words equal the row's last N-1 words, word
 // tokens[r][j + N - 1] gets probability 0: no hypothesis contains an N-gram twice.  While step < min_len, word 0 (EOS)
 // gets probability 0.  mask_unk writes entry 1 = 1e-20 (nats.py:975) BEFORE the bans, so a banned UNK ends at 0.
+// Idle rows are skipped: beam rows by the counters, sampling rows by row_done (NULL for beam search).
 __global__ void __launch_bounds__(32) beam_constrain_kernel(float* __restrict__ probs, int V, const int32_t* __restrict__ tokens,
                                                             int maxlen, int step, int k, const int32_t* __restrict__ counters,
-                                                            int no_repeat, int min_len, int mask_unk) {
+                                                            const int32_t* __restrict__ row_done, int no_repeat, int min_len,
+                                                            int mask_unk) {
     extern __shared__ int32_t s_hist[];                               // the row's `step` words
     const int row = blockIdx.x, lane = threadIdx.x;
-    if (beam_row_idle(counters, k, row)) return;
+    if (beam_row_idle(counters, k, row) || (row_done != nullptr && row_done[row] != 0)) return;
     float* p = probs + (long long)row * V;
     const int32_t* tk = tokens + (long long)row * maxlen;
     for (int t = lane; t < step; t += 32) s_hist[t] = tk[t];
@@ -344,7 +346,88 @@ int beam_constrain(cudaStream_t st, float* probs, int V, const int32_t* tokens, 
     const int n = n_src * k;
     ProfScope ps(st, K_BEAM);
     beam_constrain_kernel<<<n, 32, (size_t)step * sizeof(int32_t), st>>>(probs, V, tokens + (long long)(step & 1) * n * maxlen,
-                                                                      maxlen, step, k, counters, no_repeat, min_len, mask_unk);
+                                                                      maxlen, step, k, counters, nullptr, no_repeat, min_len,
+                                                                      mask_unk);
+    NATS_LAUNCH_OK();
+    return 0;
+}
+
+int sample_constrain(cudaStream_t st, float* probs, int V, const int32_t* tokens, int maxlen, int step, int n,
+                     const int32_t* row_done, int no_repeat, int min_len) {
+    NATS_REQUIRE(n >= 1 && n <= 65535 && step >= 0 && step < maxlen, "sample_constrain shape");
+    NATS_REQUIRE(no_repeat >= 0 && min_len >= 0, "sampling constraints must be >= 0");
+    NATS_REQUIRE(maxlen <= kBeamConstrainMaxLen, "sampling constraints need maxlen <= 12288");
+    ProfScope ps(st, K_SAMPLE);
+    beam_constrain_kernel<<<n, 32, (size_t)step * sizeof(int32_t), st>>>(probs, V, tokens, maxlen, step, 1, nullptr, row_done,
+                                                                      no_repeat, min_len, 0);
+    NATS_LAUNCH_OK();
+    return 0;
+}
+
+namespace {
+
+// Bookkeeping of one sampling step (an addition beyond the reference), one CTA per source s of the group, rows
+// [s R, s R + R).  A row that is not done takes its word v = pick[q]: tokens[q][step] = v, cost[q] -= log probs[q][v] (the
+// f_next probability, as beam search's stored cost), out_alpha[q][step] = its attention row, next_w[q] = v; v = 0 ends
+// the row with out_len[q] = step + 1.  Rows never branch, so nothing is gathered.  counters[8 + s] = finished rows of
+// source s; the last CTA to arrive (ticket counters[1], kept 0) writes the group's total to counters[0] and mirrors it
+// into host_counters[0] (pinned host memory the host polls; NULL = off).
+__global__ void __launch_bounds__(256) sample_advance_kernel(const int32_t* __restrict__ pick, const float* __restrict__ probs,
+                                                             int V, const float* __restrict__ alphaT, int Tx, int R, int maxlen,
+                                                             int step, int32_t* __restrict__ done, int32_t* __restrict__ tokens,
+                                                             float* __restrict__ cost, int32_t* __restrict__ out_len,
+                                                             float* __restrict__ out_alpha, long long* __restrict__ next_w,
+                                                             int32_t* counters, int32_t* host_counters) {
+    __shared__ int red[8];
+    const int s = blockIdx.x, tid = threadIdx.x, S = gridDim.x;
+    const long long q0 = (long long)s * R;
+    for (long long e = tid; e < (long long)R * Tx; e += 256) {         // attention rows of the rows still open
+        const long long q = q0 + e / Tx, t = e % Tx;
+        if (done[q] == 0) out_alpha[(q * maxlen + step) * Tx + t] = alphaT[q * Tx + t];
+    }
+    __syncthreads();                                                  // every read of `done` above precedes the updates
+    int nd = 0;
+    for (int j = tid; j < R; j += 256) {
+        const long long q = q0 + j;
+        if (done[q] == 0) {
+            const int v = pick[q];
+            tokens[q * maxlen + step] = v;
+            cost[q] = cost[q] - logf(probs[q * V + v]);
+            next_w[q] = v;
+            if (v == 0) { done[q] = 1; out_len[q] = step + 1; }
+        }
+        nd += done[q] != 0 ? 1 : 0;
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) nd += __shfl_xor_sync(0xffffffffu, nd, o);
+    if ((tid & 31) == 0) red[tid >> 5] = nd;
+    __syncthreads();
+    if (tid != 0) return;
+    nd = 0;
+    for (int w = 0; w < 8; ++w) nd += red[w];
+    counters[8 + s] = nd;
+    __threadfence();
+    if (atomicAdd(&counters[1], 1) != S - 1) return;
+    int total = 0;
+    for (int u = 0; u < S; ++u) total += *(volatile int32_t*)&counters[8 + u];
+    counters[1] = 0;
+    counters[0] = total;
+    if (host_counters != nullptr) {
+        *(volatile int32_t*)&host_counters[0] = total;
+        __threadfence_system();
+    }
+}
+
+}  // namespace
+
+int sample_advance(cudaStream_t st, const int32_t* pick, const float* probs, int V, const float* alphaT, int Tx, int n_src,
+                   int R, int maxlen, int step, int32_t* done, int32_t* tokens, float* cost, int32_t* out_len, float* out_alpha,
+                   long long* next_w, int32_t* counters, int32_t* host_counters) {
+    NATS_REQUIRE(n_src >= 1 && R >= 1 && (long long)n_src * R <= 65535 && step >= 0 && step < maxlen && Tx >= 1,
+                 "sample_advance shape");
+    ProfScope ps(st, K_SAMPLE);
+    sample_advance_kernel<<<n_src, 256, 0, st>>>(pick, probs, V, alphaT, Tx, R, maxlen, step, done, tokens, cost, out_len,
+                                                 out_alpha, next_w, counters, host_counters);
     NATS_LAUNCH_OK();
     return 0;
 }

@@ -162,6 +162,305 @@ __global__ void __cluster_dims__(kSmCluster, 1, 1) __launch_bounds__(kSmThreads)
     cluster.sync();                                                      // remote reads done before any CTA exits
 }
 
+// ------------------------------------------------------------------------------------------------
+// Filtered sampling (an addition beyond the reference; the rule is nats_sample_step_many's in include/nats_b200.h).
+// A cluster of 8 CTAs per row, 512 threads each; CTA r owns the contiguous slice [r*ceil(V/8), ...) of the row, which it
+// reads once from global memory into shared memory (15 KB at |V| = 30000; any |V| up to ~430000) and keeps there through
+// every pass: the weights w, then the top-k / top-p cut by radix select on the bit pattern of w (non-negative floats
+// order as unsigned integers), then the inverse CDF in vocabulary order.
+//   - Radix select: up to four 8-bit passes for top-k (bin counts) and four for top-p (bin mass).  Each CTA bins its
+//     slice in shared memory with INTEGER atomics (counts, and masses in 2^-40 fixed point of the largest weight), so the
+//     bins do not depend on the order of the adds; the 8 CTAs' bins are summed through distributed shared memory in rank
+//     order, and every CTA picks the same bin with one warp scan.  Ties at the cut value are kept in index order.
+//   - Draw: thread t owns a contiguous run of its CTA's slice; per-thread sums -> block prefix (fixed tree) -> CTA prefix
+//     (rank order) give every word a cumulative sum; the smallest kept index whose cumulative sum exceeds u*Z wins.
+// Every reduction has a fixed order, so a repeated run gives the same bits.
+// ------------------------------------------------------------------------------------------------
+constexpr int kSfCluster = 8, kSfThreads = 512, kSfWarps = kSfThreads / 32, kSfBins = 256;
+constexpr float kSfFixed = 1099511627776.f;                             // 2^40: top-p masses in fixed point
+
+// exclusive prefix of v over the block in thread order (a fixed tree: the same bits on every run); *total = block sum.
+// Contains __syncthreads(): call from uniform control flow.  s_part: kSfWarps entries of shared memory.
+template <class T>
+__device__ __forceinline__ T sf_block_prefix(T v, T* s_part, T* total) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    T inc = v;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const T y = __shfl_up_sync(0xffffffffu, inc, o);
+        if (lane >= o) inc += y;
+    }
+    T exc = __shfl_up_sync(0xffffffffu, inc, 1);
+    if (lane == 0) exc = T(0);
+    __syncthreads();                                                    // s_part may still be read by a previous call
+    if (lane == 31) s_part[warp] = inc;
+    __syncthreads();
+    T before = T(0), all = T(0);
+#pragma unroll
+    for (int w = 0; w < kSfWarps; ++w) {
+        const T t = s_part[w];
+        if (w < warp) before += t;
+        all += t;
+    }
+    *total = all;
+    return before + exc;
+}
+
+__global__ void __cluster_dims__(kSfCluster, 1, 1) __launch_bounds__(kSfThreads)
+    sample_filter_kernel(const float* __restrict__ probs, int V, const int32_t* __restrict__ row_done, int mask_unk,
+                         int ban_eos, float inv_t, int unit_t, int top_k, float top_p, uint64_t seed, int step, uint64_t row_base,
+                         int32_t* __restrict__ pick) {
+    namespace cg = cooperative_groups;
+    cg::cluster_group cluster = cg::this_cluster();
+    extern __shared__ uint32_t s_w[];                                   // this CTA's slice: p, then the bits of w
+    __shared__ uint32_t s_cnt[2][kSfBins];                              // per-pass bins (ping-pong: one cluster barrier
+    __shared__ unsigned long long s_mass[2][kSfBins];                   // per pass suffices)
+    __shared__ unsigned long long s_tot[kSfBins];                       // the cluster's bins of the current pass
+    __shared__ uint32_t s_totc[kSfBins];
+    __shared__ float s_pf[kSfWarps];
+    __shared__ int s_pi[kSfWarps];
+    __shared__ int s_bf[kSfWarps], s_bl[kSfWarps];
+    __shared__ unsigned long long s_sel[3];                             // chosen bin, quantity above it, top-p target
+    __shared__ float s_xf[2];                                           // cluster exchange slots, each written once
+    __shared__ int s_xi[5];
+    const int row = blockIdx.y;
+    if (row_done != nullptr && row_done[row] != 0) return;              // the same for all 8 CTAs of the row
+    const int rank = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int seglen = (V + kSfCluster - 1) / kSfCluster;
+    const int base = rank * seglen;
+    const int len = max(0, min(V, base + seglen) - base);
+    const float* prow = probs + (long long)row * V + base;
+
+    // 1. admissible probabilities (n-gram bans are already 0 in probs; UNK when mask_unk, EOS when ban_eos -- probs keeps
+    // their f_next values, which the bookkeeping reads), their maximum and count
+    float mx = 0.f;
+    int npos = 0;
+    for (int i = tid; i < len; i += kSfThreads) {
+        float x = __ldg(prow + i);
+        if (!(x > 0.f) || (mask_unk && base + i == 1) || (ban_eos && base + i == 0)) x = 0.f;
+        s_w[i] = __float_as_uint(x);
+        mx = fmaxf(mx, x);
+        npos += x > 0.f ? 1 : 0;
+    }
+    mx = block_max(mx, s_pf);
+    {
+        int ntot;
+        sf_block_prefix<int>(npos, s_pi, &ntot);                        // the block count (the prefix is not needed)
+        npos = ntot;
+    }
+    if (tid == 0) { s_xf[0] = mx; s_xi[0] = npos; }
+    cluster.sync();
+    float pmax = 0.f;
+    npos = 0;
+#pragma unroll
+    for (int q = 0; q < kSfCluster; ++q) {
+        pmax = fmaxf(pmax, *cluster.map_shared_rank(&s_xf[0], q));
+        npos += *cluster.map_shared_rank(&s_xi[0], q);
+    }
+
+    int result = 0;                                                     // no admissible word: the row ends with word 0
+    if (npos > 0) {
+        // 2. weights w = (p / p_max)^(1/T) (T = 1: w = p), and how many are > 0: for T < 1 the power underflows to 0 for
+        // small p (T = 0.1: p / p_max below ~3e-5), so fewer words may carry weight than are admissible
+        int nw = 0;
+        for (int i = tid; i < len; i += kSfThreads) {
+            const float x = __uint_as_float(s_w[i]);
+            const float w = unit_t ? x : (x > 0.f ? powf(x / pmax, inv_t) : 0.f);
+            s_w[i] = __float_as_uint(w);
+            nw += w > 0.f ? 1 : 0;
+        }
+        const float qs = kSfFixed / (unit_t ? pmax : 1.f);              // the largest weight -> 2^40
+        {
+            int ntot;
+            sf_block_prefix<int>(nw, s_pi, &ntot);                      // (its barriers also order the s_w stores)
+            if (tid == 0) s_xi[4] = ntot;
+        }
+        cluster.sync();
+        nw = 0;
+#pragma unroll
+        for (int q = 0; q < kSfCluster; ++q) nw += *cluster.map_shared_rank(&s_xi[4], q);   // >= 1: p_max itself has w = 1
+
+        // 3. the cut: keep every word whose key (bits of w) is > cut, and the first `ties` words (index order) with key == cut
+        uint32_t cut = 0u;
+        unsigned long long ties = 0ull;
+        int pass = 0;
+        // one radix pass over the keys below `prefix` (the top 8*d bits of the cut found so far); members: key > 0 and,
+        // when the top-k cut is on, key > kcut plus `kties` copies of kcut.  mode 0 selects by count, mode 1 by mass.
+        auto radix = [&](int mode, int d, uint32_t prefix, unsigned long long& rem, uint32_t kcut, unsigned long long kties,
+                         int total_target, float frac) -> uint32_t {
+            const int shift = 24 - 8 * d, buf = pass & 1;
+            ++pass;
+            for (int b = tid; b < kSfBins; b += kSfThreads) { s_cnt[buf][b] = 0u; s_mass[buf][b] = 0ull; }
+            __syncthreads();
+            for (int i = tid; i < len; i += kSfThreads) {
+                const uint32_t key = s_w[i];
+                if (key == 0u || key <= kcut) continue;
+                if (d > 0 && (key >> (shift + 8)) != prefix) continue;
+                const int bin = (key >> shift) & (kSfBins - 1);
+                atomicAdd(&s_cnt[buf][bin], 1u);
+                if (mode == 1) atomicAdd(&s_mass[buf][bin], (unsigned long long)__float2ull_rz(__uint_as_float(key) * qs));
+            }
+            if (tid == 0 && kties > 0ull && rank == 0 && (d == 0 || (kcut >> (shift + 8)) == prefix)) {   // the top-k ties
+                const int bin = (kcut >> shift) & (kSfBins - 1);
+                atomicAdd(&s_cnt[buf][bin], (uint32_t)kties);
+                if (mode == 1) atomicAdd(&s_mass[buf][bin], kties * (unsigned long long)__float2ull_rz(__uint_as_float(kcut) * qs));
+            }
+            cluster.sync();
+            for (int b = tid; b < kSfBins; b += kSfThreads) {
+                unsigned long long m = 0ull;
+                uint32_t c = 0u;
+#pragma unroll
+                for (int q = 0; q < kSfCluster; ++q) {
+                    c += cluster.map_shared_rank(&s_cnt[buf][0], q)[b];
+                    if (mode == 1) m += cluster.map_shared_rank(&s_mass[buf][0], q)[b];
+                }
+                s_totc[b] = c;
+                s_tot[b] = mode == 1 ? m : (unsigned long long)c;
+            }
+            __syncthreads();
+            if (warp == 0) {                                            // lane l: bins 255 - 8l .. 248 - 8l, descending
+                if (lane == 0) { s_sel[0] = 0ull; s_sel[1] = 0ull; }    // never read stale: a crossing always exists
+                __syncwarp();                                           // (want <= the members), this is only a guard
+                unsigned long long own = 0ull;
+#pragma unroll
+                for (int e = 0; e < 8; ++e) own += s_tot[kSfBins - 1 - 8 * lane - e];
+                unsigned long long inc = own;
+#pragma unroll
+                for (int o = 1; o < 32; o <<= 1) {
+                    const unsigned long long y = __shfl_up_sync(0xffffffffu, inc, o);
+                    if (lane >= o) inc += y;
+                }
+                unsigned long long want = rem;
+                if (total_target) {                                     // first top-p pass: ceil(P * total mass)
+                    const unsigned long long all = __shfl_sync(0xffffffffu, inc, 31);
+                    const unsigned long long t = (unsigned long long)ceil((double)frac * (double)all);
+                    want = t < 1ull ? 1ull : (t > all ? all : t);
+                    if (lane == 0) s_sel[2] = want;
+                }
+                const unsigned long long exc = inc - own;
+                if (exc < want && want <= inc) {                        // exactly one lane
+                    unsigned long long acc = exc;
+                    int b = kSfBins - 1 - 8 * lane;
+                    for (int e = 0; e < 7; ++e, --b) {
+                        if (acc + s_tot[b] >= want) break;
+                        acc += s_tot[b];
+                    }
+                    s_sel[0] = (unsigned long long)b;
+                    s_sel[1] = acc;
+                }
+            }
+            __syncthreads();
+            const uint32_t b = (uint32_t)s_sel[0] & (kSfBins - 1);
+            if (total_target) rem = s_sel[2];
+            rem -= s_sel[1];
+            if (d == 3) {                                               // the cut key: how many of its copies to keep
+                const unsigned long long avail = s_totc[b];
+                if (mode == 1) {
+                    const unsigned long long wq = __float2ull_rz(__uint_as_float((prefix << 8) | b) * qs);
+                    unsigned long long m = wq > 0ull ? (rem + wq - 1ull) / wq : avail;
+                    rem = m < 1ull ? 1ull : (m > avail ? avail : m);
+                } else {
+                    rem = rem > avail ? avail : rem;
+                }
+            }
+            __syncthreads();                                            // s_sel / s_tot are rewritten by the next pass
+            return (prefix << 8) | b;
+        };
+        if (top_k >= 1 && top_k < nw) {                                 // else every word of positive weight is kept
+            unsigned long long rem = (unsigned long long)top_k;
+            uint32_t prefix = 0u;
+            for (int d = 0; d < 4; ++d) prefix = radix(0, d, prefix, rem, 0u, 0ull, 0, 0.f);
+            cut = prefix; ties = rem;
+        }
+        if (top_p < 1.f) {
+            const uint32_t kcut = ties > 0ull ? cut : 0u;
+            const unsigned long long kties = ties;
+            unsigned long long rem = 0ull;
+            uint32_t prefix = 0u;
+            for (int d = 0; d < 4; ++d) prefix = radix(1, d, prefix, rem, kcut, kties, d == 0, top_p);
+            cut = prefix; ties = rem;
+        }
+
+        // 4. tie ranks at the cut key, in vocabulary order (only when a cut is on)
+        const int per = (len + kSfThreads - 1) / kSfThreads;
+        const int r0 = min(len, tid * per), r1 = min(len, r0 + per);
+        long long trank = 0;
+        if (ties > 0ull) {
+            int c = 0;
+            for (int i = r0; i < r1; ++i) c += s_w[i] == cut ? 1 : 0;
+            int ctot;
+            const int cex = sf_block_prefix<int>(c, s_pi, &ctot);
+            if (tid == 0) s_xi[1] = ctot;
+            cluster.sync();
+            long long off = 0;
+            for (int q = 0; q < rank; ++q) off += *cluster.map_shared_rank(&s_xi[1], q);
+            trank = off + cex;
+        }
+        auto kept = [&](uint32_t key, long long& tr) -> bool {
+            if (key == cut && key != 0u) return (unsigned long long)(tr++) < ties;
+            return key > cut;
+        };
+
+        // 5. kept sums in vocabulary order: thread run -> block prefix -> CTA prefix in rank order
+        float s = 0.f;
+        int last = -1;
+        {
+            long long tr = trank;
+            for (int i = r0; i < r1; ++i) {
+                const uint32_t key = s_w[i];
+                if (kept(key, tr)) { s += __uint_as_float(key); last = base + i; }
+            }
+        }
+        float ctot;
+        const float sex = sf_block_prefix<float>(s, s_pf, &ctot);
+        if (tid == 0) s_xf[1] = ctot;
+        cluster.sync();
+        float off = 0.f, Z = 0.f;
+#pragma unroll
+        for (int q = 0; q < kSfCluster; ++q) {
+            const float t = *cluster.map_shared_rank(&s_xf[1], q);
+            if (q < rank) off += t;
+            Z += t;
+        }
+
+        // 6. the draw: the smallest kept index v with u*Z < (cumulative kept weight through v); rounding: the last kept word
+        const float uz = uniform01(seed, (uint64_t)step, row_base + (uint64_t)row) * Z;
+        int found = 0x7fffffff;
+        if (Z > 0.f) {
+            float c = off + sex;
+            long long tr = trank;
+            for (int i = r0; i < r1; ++i) {
+                const uint32_t key = s_w[i];
+                if (kept(key, tr)) {
+                    c += __uint_as_float(key);
+                    if (uz < c) { found = base + i; break; }
+                }
+            }
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {                              // block min of `found`, max of `last`
+            found = min(found, __shfl_xor_sync(0xffffffffu, found, o));
+            last = max(last, __shfl_xor_sync(0xffffffffu, last, o));
+        }
+        if (lane == 0) { s_bf[warp] = found; s_bl[warp] = last; }
+        __syncthreads();
+        int bf = 0x7fffffff, bl = -1;
+#pragma unroll
+        for (int w = 0; w < kSfWarps; ++w) { bf = min(bf, s_bf[w]); bl = max(bl, s_bl[w]); }
+        if (tid == 0) { s_xi[2] = bf; s_xi[3] = bl; }
+        cluster.sync();
+        int gf = 0x7fffffff, gl = -1;
+#pragma unroll
+        for (int q = 0; q < kSfCluster; ++q) {
+            gf = min(gf, *cluster.map_shared_rank(&s_xi[2], q));
+            gl = max(gl, *cluster.map_shared_rank(&s_xi[3], q));
+        }
+        if (Z > 0.f && gl >= 0) result = gf != 0x7fffffff ? gf : gl;
+    }
+    if (rank == 0 && tid == 0) pick[row] = result;
+    cluster.sync();                                                     // remote reads done before any CTA exits
+}
+
 
 // ------------------------------------------------------------------------------------------------
 // Few rows x narrow output (f_next's readout hidden layer, nats.py:850-857):
@@ -364,6 +663,22 @@ int softmax_sample_rows(cudaStream_t st, const float* logits, int rows, int V, f
         return 0;
     }
     softmax_sample_kernel<<<rows, kRowThreads, 0, st>>>(logits, V, probs, sample, seed, step);
+    NATS_LAUNCH_OK();
+    return 0;
+}
+
+int sample_filter(cudaStream_t st, const float* probs, int rows, int V, const int32_t* row_done, int mask_unk, int ban_eos,
+                  float temperature, int top_k, float top_p, uint64_t seed, int step, uint64_t row_base, int32_t* pick) {
+    NATS_REQUIRE(rows >= 1 && rows <= 65535 && V >= 2, "sample_filter shape");
+    NATS_REQUIRE(temperature > 0.f && top_k >= 0 && top_p > 0.f && top_p <= 1.f, "sample_filter arguments");
+    const size_t smem = (size_t)((V + kSfCluster - 1) / kSfCluster) * sizeof(uint32_t);
+    if (smem > 48 * 1024) {                                                // beyond the default: opt in (up to the SM's limit)
+        NATS_CUDA_OK(cudaFuncSetAttribute(sample_filter_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    }
+    ProfScope ps(st, K_SAMPLE, 0.0, 4.0 * rows * V);
+    sample_filter_kernel<<<dim3(kSfCluster, rows), kSfThreads, smem, st>>>(probs, V, row_done, mask_unk, ban_eos,
+                                                                          1.f / temperature, temperature == 1.f ? 1 : 0, top_k,
+                                                                          top_p, seed, step, row_base, pick);
     NATS_LAUNCH_OK();
     return 0;
 }

@@ -28,6 +28,7 @@ enum KClass {
     K_TC_GEMM_SKINNY,    // wgmma 3xTF32, N side <= 64 (the batch, roles swapped)
     K_ENC_PERSIST_FWD,   // persistent weight-stationary wgmma bidirectional encoder recurrence (one launch per pass)
     K_ENC_PERSIST_BWD,
+    K_SAMPLE,            // filtered sampling: bans, draw and bookkeeping of nats_sample_step_many
     K_COUNT
 };
 

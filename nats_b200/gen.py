@@ -7,6 +7,13 @@ the visible GPUs (one model replica per process, gen.py:78-85) and `-p 1` decode
 
 Two long options go beyond the reference, both off by default: `--no-repeat-ngram N` keeps every summary free of a repeated
 N-gram and `--min-len L` lets no summary end before L words (nats.gen_sample's no_repeat_ngram / min_len).
+
+Sampling instead of beam search, also beyond the reference: `--sample R` draws R summaries of every line (nats.sample_many)
+shaped by `--temperature T`, `--top-k K` and `--top-p P`, with the draws fixed by `--seed S`, and prints the one of lowest
+cost (normalised by length with -n).  The distraction factors -l / -x / -s belong to beam search and are refused with it;
+the two constraints apply.  A line's draws depend only on the seed and its position in the file, not on -p.
+
+    python -m nats_b200.gen -n -p 2 --sample 10 --top-p 0.9 --seed 7 model.npz dictionary.pkl source.txt out.txt
 """
 import argparse
 import multiprocessing as mp
@@ -31,7 +38,8 @@ CHUNK = 16     # sentences encoded per f_init launch (and per queue item of a wo
 class _Translator(object):
     """one model replica: parameters from the checkpoint, sampler, beam search (gen.py:15-48)"""
 
-    def __init__(self, model, options, k, normalize, kl_factor, ctx_factor, state_factor, no_repeat_ngram=0, min_len=0):
+    def __init__(self, model, options, k, normalize, kl_factor, ctx_factor, state_factor, no_repeat_ngram=0, min_len=0,
+                 sampling=None):
         from . import nats
         self.nats = nats
         params = nats.load_params(model, nats.init_params(options))
@@ -40,6 +48,7 @@ class _Translator(object):
         self.options, self.k, self.normalize = options, k, normalize
         self.factors = (kl_factor, ctx_factor, state_factor)
         self.constraints = dict(no_repeat_ngram=no_repeat_ngram, min_len=min_len)
+        self.sampling = sampling or {}                           # sample_many's keywords; empty: beam search
 
     def prefetch(self, seqs):
         """encode the next sentences in ONE encoder launch (f_init is most of a short summary's time); optional"""
@@ -47,8 +56,15 @@ class _Translator(object):
         if pf is not None and self.k <= 32 and os.environ.get('NATS_DEVICE_BEAM', '1') != '0':
             pf([numpy.array(s, dtype='int64') for s in seqs])
 
-    def many(self, seqs):
-        """a chunk of sentences: encoders in one launch, several beam searches in flight (nats.gen_sample_many)"""
+    def many(self, seqs, index_base=0):
+        """a chunk of sentences: encoders in one launch, several beam searches in flight (nats.gen_sample_many); with
+        --sample, R samples of each (nats.sample_many), the chunk's first sentence being line `index_base` of the file"""
+        if self.sampling:
+            outs = self.nats.sample_many(self.tparams, self.f_init, self.f_next, [numpy.array(s, dtype='int64') for s in seqs],
+                                         self.options, maxlen=100, use_unk=True, index_base=index_base,
+                                         concurrency=int(os.environ.get('NATS_GEN_STREAMS', '12')), chunk=CHUNK,
+                                         **dict(self.constraints, **self.sampling))
+            return [self._best(*o) for o in outs]
         kl, cf, sf = self.factors
         outs = self.nats.gen_sample_many(self.tparams, self.f_init, self.f_next, [numpy.array(s, dtype='int64') for s in seqs],
                                          self.options, trng=None, k=self.k, maxlen=100, use_unk=True, kl_factor=kl,
@@ -74,25 +90,42 @@ class _Translator(object):
 
 
 def translate_model(queue, rqueue, pid, model, options, k, normalize, kl_factor, ctx_factor, state_factor, no_repeat_ngram=0,
-                    min_len=0):
+                    min_len=0, sampling=None):
     import torch
     n_dev = max(torch.cuda.device_count(), 1)
     os.environ['LOCAL_RANK'] = str(pid % n_dev)               # the engine binds to this device
     torch.cuda.set_device(pid % n_dev)
-    tr = _Translator(model, options, k, normalize, kl_factor, ctx_factor, state_factor, no_repeat_ngram, min_len)
+    tr = _Translator(model, options, k, normalize, kl_factor, ctx_factor, state_factor, no_repeat_ngram, min_len, sampling)
     while True:
         req = queue.get()
         if req is None:
             break
         print(pid, '-', req[0][0], '..', req[-1][0])            # a chunk of jobs
-        for (idx, _), (seq, pos) in zip(req, tr.many([x for _, x in req])):
+        for (idx, _), (seq, pos) in zip(req, tr.many([x for _, x in req], req[0][0])):
             rqueue.put((idx, seq, pos))
 
 
+def _sampling_args(sample, temperature, top_k, top_p, seed, kl_factor, ctx_factor, state_factor):
+    """--sample and its options -> sample_many's keywords ({} = beam search); ValueError for a bad combination"""
+    if sample < 0:
+        raise ValueError('--sample must be >= 0 (0 = beam search)')
+    if sample == 0:
+        if (temperature, top_k, top_p, seed) != (1., 0, 1., 1234):
+            raise ValueError('--temperature, --top-k, --top-p and --seed need --sample R')
+        return {}
+    if kl_factor or ctx_factor or state_factor:
+        raise ValueError('-l / -x / -s re-rank beam search; they do not apply with --sample')
+    from . import nats
+    R, _, temperature, top_k, top_p, seed, _, _, _ = nats._check_sampling(sample, 100, temperature, top_k, top_p, seed, 0, 0,
+                                                                           0, CHUNK)
+    return dict(n_samples=R, temperature=temperature, top_k=top_k, top_p=top_p, seed=seed)
+
+
 def main(model, dictionary, source_file, saveto, k=5, normalize=False, n_process=5, chr_level=False, kl_factor=0,
-         ctx_factor=0, state_factor=0, no_repeat_ngram=0, min_len=0):
+         ctx_factor=0, state_factor=0, no_repeat_ngram=0, min_len=0, sample=0, temperature=1., top_k=0, top_p=1., seed=1234):
     if no_repeat_ngram < 0 or min_len < 0:
         raise ValueError('--no-repeat-ngram and --min-len must be >= 0 (0 = off)')
+    sampling = _sampling_args(sample, temperature, top_k, top_p, seed, kl_factor, ctx_factor, state_factor)
     options = _load_pickle('%s.pkl' % model)
     word_dict = _load_pickle(dictionary)
     word_idict = dict((vv, kk) for kk, vv in word_dict.items())
@@ -112,16 +145,16 @@ def main(model, dictionary, source_file, saveto, k=5, normalize=False, n_process
     print('Inferece ', source_file, '...')
     trans, pos = [None] * n_samples, [None] * n_samples
     if n_process <= 1:
-        tr = _Translator(model, options, k, normalize, kl_factor, ctx_factor, state_factor, no_repeat_ngram, min_len)
+        tr = _Translator(model, options, k, normalize, kl_factor, ctx_factor, state_factor, no_repeat_ngram, min_len, sampling)
         for lo in range(0, len(jobs), CHUNK):
-            for (idx, _), (seq, p_) in zip(jobs[lo:lo + CHUNK], tr.many([j[1] for j in jobs[lo:lo + CHUNK]])):
+            for (idx, _), (seq, p_) in zip(jobs[lo:lo + CHUNK], tr.many([j[1] for j in jobs[lo:lo + CHUNK]], lo)):
                 trans[idx], pos[idx] = seq, p_
             print('Sample ', min(lo + CHUNK, n_samples), '/', n_samples, ' Done')
     else:
         ctx = mp.get_context('spawn')                          # CUDA contexts do not survive fork
         queue, rqueue = ctx.Queue(), ctx.Queue()
         procs = [ctx.Process(target=translate_model, args=(queue, rqueue, midx, model, options, k, normalize, kl_factor,
-                                                           ctx_factor, state_factor, no_repeat_ngram, min_len))
+                                                           ctx_factor, state_factor, no_repeat_ngram, min_len, sampling))
                  for midx in range(n_process)]
         for p in procs:
             p.start()
@@ -164,6 +197,13 @@ if __name__ == '__main__':
                         help='no summary contains the same N-gram twice (0 = off)')
     parser.add_argument('--min-len', type=int, default=0, metavar='L',
                         help='no summary ends before L words (0 = off)')
+    parser.add_argument('--sample', type=int, default=0, metavar='R',
+                        help='draw R summaries of every line and print the one of lowest cost (0 = beam search)')
+    parser.add_argument('--temperature', type=float, default=1., metavar='T', help='sampling temperature (> 0)')
+    parser.add_argument('--top-k', type=int, default=0, metavar='K', help='sample among the K most probable words (0 = off)')
+    parser.add_argument('--top-p', type=float, default=1., metavar='P',
+                        help='sample among the most probable words holding P of the mass (1 = off)')
+    parser.add_argument('--seed', type=int, default=1234, metavar='S', help='seed of the draws')
     parser.add_argument('model', type=str)
     parser.add_argument('dictionary', type=str)
     parser.add_argument('source', type=str)
@@ -171,4 +211,5 @@ if __name__ == '__main__':
     args = parser.parse_args()
     main(args.model, args.dictionary, args.source, args.saveto, k=args.k, normalize=args.n, n_process=args.p,
          chr_level=args.c, kl_factor=args.l, ctx_factor=args.x, state_factor=args.s, no_repeat_ngram=args.no_repeat_ngram,
-         min_len=args.min_len)
+         min_len=args.min_len, sample=args.sample, temperature=args.temperature, top_k=args.top_k, top_p=args.top_p,
+         seed=args.seed)

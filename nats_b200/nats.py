@@ -1145,7 +1145,35 @@ def _tile_ctx(ctx0, live_k):
     return numpy.tile(ctx0, [live_k, 1])
 
 
-class _DeviceBeam(object):
+class _DeviceGroup(object):
+    """What the device-resident decoders of a group of sources share: each step is ONE foreign call on a prebuilt argument
+    struct per ping-pong parity (self.one_call), and the host learns of the group's progress through one 4-byte flag,
+    host_np[_flag], that the step's last kernel mirrors into pinned host memory.  The flag is read two steps late (after
+    that step's event), so the GPU queue never drains; the group is over at maxlen or once the flag reaches _flag_done."""
+
+    def _next_step(self):
+        """-> the index of the step to issue now, or None when the group is over"""
+        ii = self.ii
+        if ii >= self.maxlen:
+            return None
+        if ii >= 2:
+            self.events[ii & 1].synchronize()                 # step ii-2 is through: its flag is in host memory
+            if self.host_np[self._flag] >= self._flag_done:
+                self.ii = self.maxlen
+                return None
+        self.ii = ii + 1
+        return ii
+
+    def _one_call(self, fn, name, ii):
+        rc = fn(*self.one_call[ii & 1], ii)
+        if rc != 0:
+            self.check(rc, name)
+        self.eng.launches += 1
+        self.events[ii & 1].record(self.tstream)
+        return True
+
+
+class _DeviceBeam(_DeviceGroup):
     """Beam search with every piece of bookkeeping on the device (SURVEY 8(f).1, replaces the host loop of
     nats.py:1001-1066), for a GROUP of S source sentences at once: per step ONE f_next on S*k rows (row s*k + j is row j of
     sentence s and attends to its own source; rows >= live_k of a sentence are ignored), the distraction penalties, a
@@ -1273,6 +1301,7 @@ class _DeviceBeam(object):
             a.hist_ctx_out = hist_ctx[c ^ 1].data_ptr() if distract else None
             a.hist_state_out = hist_state[c ^ 1].data_ptr() if distract else None
             one_call.append((eng.ctx, stream, ctypes.byref(dims_), ctypes.byref(m)))
+        _flag, _flag_done = 5, S                                 # host_cnt[5]: sentences that are done
         # every local becomes an attribute: step() / result() use a dozen of them, and ALL the tensors above must outlive the
         # search because their addresses sit in the prebuilt argument structs (a tensor dropped here would be a dangling pointer)
         keep = dict(locals())
@@ -1283,25 +1312,12 @@ class _DeviceBeam(object):
     def step(self):
         """issue iteration self.ii; False when the search has ended (every sentence retired all its hypotheses or
         maxlen was reached)"""
-        ii, maxlen, torch = self.ii, self.maxlen, self.torch
-        if ii >= maxlen:
+        ii = self._next_step()
+        if ii is None:
             return False
-        cur = ii & 1
-        events = self.events
-        if ii >= 2:
-            events[cur].synchronize()                         # step ii-2 is through: its counters are in host memory
-            if self.host_np[5] >= self.S:
-                self.ii = maxlen
-                return False
-        self.ii = ii + 1
-        eng = self.eng
         if self._trace is None:
-            rc = self.lib.nats_beam_step_many(*self.one_call[cur], ii)
-            if rc != 0:
-                self.check(rc, 'nats_beam_step_many')
-            eng.launches += 1
-            events[cur].record(self.tstream)
-            return True
+            return self._one_call(self.lib.nats_beam_step_many, 'nats_beam_step_many', ii)
+        maxlen, torch, cur, events, eng = self.maxlen, self.torch, ii & 1, self.events, self.eng
         lib, check, k = self.lib, self.check, self.k
         with torch.cuda.stream(self.tstream):
             self.step_next[cur]()
@@ -1402,11 +1418,23 @@ def gen_sample_many(tparams, f_init, f_next, xs, options, trng=None, k=5, maxlen
     dim 1000).  no_repeat_ngram / min_len: the output constraints of gen_sample."""
     no_repeat_ngram, min_len = _check_constraints(no_repeat_ngram, min_len)
     eng = f_next.engine
-    torch = eng.torch
     if k > 32 or getattr(f_init, 'device', None) is None or os.environ.get('NATS_DEVICE_BEAM', '1') == '0':
         return [gen_sample(tparams, f_init, f_next, numpy.asarray(x).reshape(-1, 1), options, trng, k, maxlen, False, False,
                            use_unk, kl_factor, ctx_factor, state_factor, no_repeat_ngram=no_repeat_ngram, min_len=min_len)
                 for x in xs]
+    return _drive_groups(eng, xs, chunk, concurrency,
+                         lambda grp, first, slot, stream: _DeviceBeam(f_init, f_next, grp, k, maxlen, use_unk, kl_factor,
+                                                                      ctx_factor, state_factor, None, slot, stream,
+                                                                      no_repeat_ngram, min_len))
+
+
+def _drive_groups(eng, xs, chunk, concurrency, make):
+    """The driver of gen_sample_many and sample_many: every `chunk` consecutive sources of the list xs form one group,
+    make(group, index of its first source, workspace slot, stream) -> a _DeviceGroup that has set itself up on `stream`.
+    `concurrency` groups are in flight, each on its own CUDA stream with its own workspace slot; their steps are issued in
+    turn until each is over, and a finished group's stream takes the next one.  -> the groups' results, one per source, in
+    order."""
+    torch = eng.torch
     chunk = max(1, int(chunk))
     streams = getattr(eng, '_beam_streams', None)
     if streams is None:
@@ -1421,8 +1449,7 @@ def gen_sample_many(tparams, f_init, f_next, xs, options, trng=None, k=5, maxlen
         nonlocal nxt
         grp = [numpy.asarray(x).reshape(-1) for x in xs[nxt:nxt + chunk]]
         streams[slot].wait_stream(main)                           # whatever the current stream queued comes first
-        b = _DeviceBeam(f_init, f_next, grp, k, maxlen, use_unk, kl_factor, ctx_factor, state_factor, None, slot + 1,
-                        streams[slot], no_repeat_ngram, min_len)
+        b = make(grp, nxt, slot + 1, streams[slot])
         active[slot] = (nxt, b)
         nxt += len(grp)
         b.step()
@@ -1442,6 +1469,156 @@ def gen_sample_many(tparams, f_init, f_next, xs, options, trng=None, k=5, maxlen
             res = b.result()
             results[idx:idx + len(res)] = res
     return results
+
+
+class _DeviceSample(_DeviceGroup):
+    """Filtered sampling (an addition beyond the reference) of a GROUP of S sources with R samples each, on the device: per
+    step ONE nats_sample_step_many -- f_next on the S*R rows (row s*R + j attends to source s), the output constraints
+    when one is on, the filtered draw and the bookkeeping.  Rows never branch, so the state / accumulator rows simply
+    ping-pong.  The host polls the group's count of finished rows two steps late (see _DeviceGroup) and copies tokens,
+    costs, lengths and attention rows back once at the end.  row_base = global row id of the group's first row."""
+
+    def __init__(self, f_init, f_next, xs, R, maxlen, use_unk, temperature, top_k, top_p, no_repeat_ngram, min_len, seed,
+                 row_base, slot=0, stream=None):
+        torch = f_next.engine.torch
+        self.tstream = stream if stream is not None else torch.cuda.current_stream(f_next.engine.device)
+        with torch.cuda.stream(self.tstream):
+            self._setup(f_init, f_next, xs, R, maxlen, use_unk, temperature, top_k, top_p, no_repeat_ngram, min_len, seed,
+                        row_base, slot)
+
+    def _setup(self, f_init, f_next, xs, R, maxlen, use_unk, temperature, top_k, top_p, no_repeat_ngram, min_len, seed,
+               row_base, slot):
+        eng = f_next.engine
+        torch = eng.torch
+        lib = eng.lib
+        V, W, D, A = f_next.dims
+        C = 2 * D
+        S = len(xs)
+        n = S * R
+        init_state, ctx_d, pctx_d, src_lens = f_init.group(xs)        # device tensors [S, D], [Tx, S, C], [Tx, S, A]
+        Tx = int(ctx_d.shape[0])
+        dev = eng.device
+        f32 = dict(dtype=torch.float32, device=dev)
+        i32 = dict(dtype=torch.int32, device=dev)
+        state = [init_state.reshape(S, 1, D).expand(S, R, D).reshape(n, D).contiguous(), torch.empty((n, D), **f32)]
+        acc_ctx = [torch.zeros((n, C), **f32) for _ in range(2)]
+        acc_alpha = [torch.zeros((n, Tx), **f32) for _ in range(2)]
+        probs, alphaT, ctxs = torch.empty((n, V), **f32), torch.empty((n, Tx), **f32), torch.empty((n, C), **f32)
+        src_len_h = torch.tensor(src_lens, dtype=torch.int32).pin_memory()
+        src_len = src_len_h.to(dev, non_blocking=True)
+        next_w = torch.full((n,), -1, dtype=torch.int64, device=dev)          # BOS marker -> zero embedding
+        pick, done = torch.zeros((n,), **i32), torch.zeros((n,), **i32)
+        tokens = torch.zeros((n, maxlen), **i32)
+        cost = torch.zeros((n,), **f32)
+        out_len = torch.full((n,), maxlen, **i32)
+        out_alpha = torch.zeros((n, maxlen, Tx), **f32)
+        counters = torch.zeros((8 + S,), **i32)
+        host_cnt = torch.zeros(8, dtype=torch.int32).pin_memory()
+        host_np = host_cnt.numpy()
+        events = [torch.cuda.Event() for _ in range(2)]
+        stream = ctypes.c_void_p(self.tstream.cuda_stream)
+        ws_for, tp_, dims_ = f_next.beam_env
+        ws_t, ws_bytes = ws_for(Tx, n, slot)
+        one_call = []
+        for c in (0, 1):
+            m = _lib.SampleStepMany()
+            m.params, m.next_w, m.ctx, m.pctx = tp_.flat.data_ptr(), next_w.data_ptr(), ctx_d.data_ptr(), pctx_d.data_ptr()
+            m.src_len = src_len.data_ptr()
+            m.Tx, m.n_src, m.n_samples, m.maxlen = Tx, S, R, maxlen
+            m.use_unk, m.top_k, m.no_repeat_ngram, m.min_len = 1 if use_unk else 0, top_k, no_repeat_ngram, min_len
+            m.temperature, m.top_p, m.seed, m.row_base = temperature, top_p, seed, row_base
+            m.ws, m.ws_bytes = ws_t.data_ptr(), ws_bytes
+            m.state_in, m.acc_ctx_in, m.acc_alpha_in = state[c].data_ptr(), acc_ctx[c].data_ptr(), acc_alpha[c].data_ptr()
+            m.state_out, m.acc_ctx_out = state[c ^ 1].data_ptr(), acc_ctx[c ^ 1].data_ptr()
+            m.acc_alpha_out = acc_alpha[c ^ 1].data_ptr()
+            m.probs, m.alphaT, m.ctxs = probs.data_ptr(), alphaT.data_ptr(), ctxs.data_ptr()
+            m.pick, m.done, m.tokens, m.cost = pick.data_ptr(), done.data_ptr(), tokens.data_ptr(), cost.data_ptr()
+            m.out_len, m.out_alpha = out_len.data_ptr(), out_alpha.data_ptr()
+            m.counters, m.host_counters = counters.data_ptr(), host_cnt.data_ptr()
+            one_call.append((eng.ctx, stream, ctypes.byref(dims_), ctypes.byref(m)))
+        _flag, _flag_done = 0, n                                 # host_cnt[0]: rows that are done
+        check = _lib.check
+        # as in _DeviceBeam: every tensor above must outlive the group (their addresses sit in the argument structs)
+        keep = dict(locals())
+        keep.pop('self')
+        self.__dict__.update(keep)
+        self.ii = 0
+
+    def step(self):
+        """issue step self.ii; False when the group is over (every row ended or maxlen was reached)"""
+        ii = self._next_step()
+        if ii is None:
+            return False
+        return self._one_call(self.lib.nats_sample_step_many, 'nats_sample_step_many', ii)
+
+    def result(self):
+        """per source, gen_sample's three lists for its R samples in order; attention rows cut to the source's length"""
+        with self.torch.cuda.stream(self.tstream):
+            self.tstream.synchronize()
+            tok, cost, lens = self.tokens.cpu().numpy(), self.cost.cpu().numpy(), self.out_len.cpu().numpy()
+            al = self.out_alpha.cpu().numpy()
+        res = []
+        for s in range(self.S):
+            Ls = self.src_lens[s]
+            samples, costs, alphas = [], [], []
+            for q in range(s * self.R, (s + 1) * self.R):
+                L = int(lens[q])
+                samples.append([int(t) for t in tok[q, :L]])
+                costs.append(numpy.float32(cost[q]))
+                alphas.append(list(al[q, :L, :Ls].copy()))
+            res.append((samples, costs, alphas))
+        return res
+
+
+def _check_sampling(n_samples, maxlen, temperature, top_k, top_p, seed, index_base, no_repeat_ngram, min_len, chunk):
+    """the arguments of sample_many, checked before anything is launched (nats_sample_step_many refuses the same)"""
+    no_repeat_ngram, min_len = _check_constraints(no_repeat_ngram, min_len)
+    if int(n_samples) != n_samples or n_samples < 1:
+        raise ValueError('n_samples must be an integer >= 1, got %r' % (n_samples,))
+    if int(maxlen) != maxlen or maxlen < 1:
+        raise ValueError('maxlen must be an integer >= 1, got %r' % (maxlen,))
+    temperature, top_p = float(temperature), float(top_p)
+    if not temperature > 0.:                                  # NaN fails too
+        raise ValueError('temperature must be > 0, got %r' % temperature)
+    if int(top_k) != top_k or top_k < 0:
+        raise ValueError('top_k must be an integer >= 0 (0 = off), got %r' % (top_k,))
+    if not 0. < top_p <= 1.:
+        raise ValueError('top_p must be in (0, 1] (1 = off), got %r' % top_p)
+    if int(seed) != seed or not 0 <= seed < 2 ** 64:
+        raise ValueError('seed must be an integer in [0, 2^64), got %r' % (seed,))
+    if int(index_base) != index_base or index_base < 0:
+        raise ValueError('index_base must be an integer >= 0, got %r' % (index_base,))
+    if max(1, int(chunk)) * int(n_samples) > 65535:
+        raise ValueError('chunk x n_samples = %d rows per group; at most 65535' % (max(1, int(chunk)) * int(n_samples)))
+    if (no_repeat_ngram or min_len) and maxlen > 12288:
+        raise ValueError('no_repeat_ngram / min_len need maxlen <= 12288')
+    return (int(n_samples), int(maxlen), temperature, int(top_k), top_p, int(seed), int(index_base), no_repeat_ngram,
+            min_len)
+
+
+def sample_many(tparams, f_init, f_next, xs, options, n_samples=5, maxlen=30, temperature=1., top_k=0, top_p=1.,
+                use_unk=True, no_repeat_ngram=0, min_len=0, seed=1234, index_base=0, concurrency=12, chunk=16):
+    """Filtered sampling (an addition beyond the reference) of a LIST of source sentences: R = n_samples independent
+    summaries of each, drawn on the device -> per source gen_sample's three lists (samples, costs, alphas), each of length R
+    in sample order, so gen's selection rule applies unchanged.
+
+    Each step runs f_next exactly as the grouped beam search does (no distraction re-ranking), bans words by use_unk /
+    min_len / no_repeat_ngram (the rule of gen_sample's constraints), weights the others w = (p / p_max)^(1 / temperature),
+    keeps the top_k most probable (0 = off) and then the smallest set holding top_p of their weight (1 = off), and draws
+    with the counter-based uniform of (seed, step, global row id (index_base + i) * R + j).  A sample ends with EOS (kept in
+    it) or at maxlen; its cost is the sum of -log p of its words under the unfiltered f_next probabilities, as beam search's.
+    The draws of a source do not depend on chunk, concurrency, its neighbours or the process that drew them: a caller that
+    splits a list passes each part's global start as index_base.  The exact rule is nats_sample_step_many's
+    (include/nats_b200.h).  Groups of `chunk` sources run `concurrency` at a time on their own streams, as in
+    gen_sample_many.  Invalid arguments raise ValueError before anything is launched; there is no host fallback."""
+    (R, maxlen, temperature, top_k, top_p, seed, index_base, no_repeat_ngram,
+     min_len) = _check_sampling(n_samples, maxlen, temperature, top_k, top_p, seed, index_base, no_repeat_ngram, min_len, chunk)
+    if getattr(f_init, 'group', None) is None or getattr(f_next, 'beam_env', None) is None:
+        raise ValueError('sample_many needs the f_init / f_next of build_sampler')
+    return _drive_groups(f_next.engine, xs, chunk, concurrency,
+                         lambda grp, first, slot, stream: _DeviceSample(f_init, f_next, grp, R, maxlen, use_unk, temperature,
+                                                                        top_k, top_p, no_repeat_ngram, min_len, seed,
+                                                                        (index_base + first) * R, slot, stream))
 
 
 def gen_sample(tparams, f_init, f_next, x, options, trng=None, k=1, maxlen=30, stochastic=True, argmax=False,
