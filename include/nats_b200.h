@@ -36,6 +36,7 @@ extern "C" {
 #define NATS_NUM_PARAMS 43          /* nats.py:613-654 */
 #define NATS_GRAD_TAIL 32           /* extra floats after the parameter area of a gradient buffer:
                                        [0] = sum_b cost_b * scale (so one allreduce carries cost + grads) */
+#define NATS_ROUGE_MAX_CAP 4096     /* nats_rouge_f: largest ref_cap + cand_cap */
 
 typedef struct nats_ctx nats_ctx_t; /* opaque: device id, SM count, small device scratch */
 
@@ -97,6 +98,23 @@ int nats_train_bwd_begin(nats_ctx_t* ctx, void* stream, const nats_dims_t* dims,
 int nats_train_bwd_finish(nats_ctx_t* ctx, void* stream, const nats_dims_t* dims, const float* params,
                           const int64_t* x, const float* x_mask, const int64_t* y, const float* y_mask,
                           int Tx, int Ty, int B, void* ws, int64_t ws_bytes, float scale, float* grads);
+
+/* Per-sample weighted backward (an addition beyond the reference; self-critical training weighs each sampled summary by
+ * its reward's advantage, some weights negative).  The arguments of nats_train_bwd / nats_train_bwd_begin plus
+ * weight [B] (device float32; NULL is an error: the unweighted calls are the way to train without weights):
+ *   grads = d( scale * sum_b weight[b] * cost_b ) / d params,   grads[total_floats] = scale * sum_b weight[b] * cost_b.
+ * The backward is linear in d logits, so the weight enters only there (row t*B + b of d logits is scaled by weight[b]) and
+ * in the cost tail; every product after it is the unweighted one.  nats_train_bwd_finish completes either half unchanged,
+ * and nats_train_fwd's per-sample cost stays the unweighted NLL.  A weight that is a power of two (or its negative) scales
+ * every gradient by exactly that factor, except the Wemb scatter, whose float atomics have no fixed order. */
+int nats_train_bwd_weighted(nats_ctx_t* ctx, void* stream, const nats_dims_t* dims, const float* params,
+                            const int64_t* x, const float* x_mask, const int64_t* y, const float* y_mask,
+                            int Tx, int Ty, int B, void* ws, int64_t ws_bytes, float scale, const float* weight,
+                            float* grads);
+int nats_train_bwd_begin_weighted(nats_ctx_t* ctx, void* stream, const nats_dims_t* dims, const float* params,
+                                  const int64_t* x, const float* x_mask, const int64_t* y, const float* y_mask,
+                                  int Tx, int Ty, int B, void* ws, int64_t ws_bytes, float scale, const float* weight,
+                                  float* grads);
 
 /* Finer-grained pieces of the same graph (SURVEY 8(b)); all operate on the same workspace. */
 int nats_encoder_fwd(nats_ctx_t* ctx, void* stream, const nats_dims_t* dims, const float* params,
@@ -348,6 +366,21 @@ typedef struct nats_sample_step_many {
     int32_t* counters; int32_t* host_counters;
 } nats_sample_step_many_t;
 int nats_sample_step_many(nats_ctx_t* ctx, void* stream, const nats_dims_t* dims, const nats_sample_step_many_t* a, int step);
+
+/* ---------------------------------------------------------------- rewards ----------------------- */
+/* ROUGE of token ids (an addition beyond the reference; the reward of self-critical training): out [3, n] (device float32)
+ * = the ROUGE-1, ROUGE-2 and ROUGE-L F of candidate row r against reference row r / rows_per_ref, n = n_ref * rows_per_ref.
+ *   cand [n, cand_cap] int32 with cand_len [n], ref [n_ref, ref_cap] int32 with ref_len [n_ref] (all device arrays).
+ *   A row's words are its first min(len, cap) entries (len clamped to [0, cap]) up to the first 0 (EOS, excluded).
+ *   UNK (1) matches nothing, UNK included, but counts in the lengths.  Hits: ROUGE-N, the clipped counts
+ *   sum_g min(c_ref(g), c_cand(g)) of ROUGE.pl (N = 1, 2); ROUGE-L, the length of the longest common subsequence.
+ *   F = (float)(2 h) / (float)(m + c), h the hits, m and c the reference's and the candidate's n-gram counts
+ *   max(0, len - N + 1) (ROUGE-L: the lengths); F = 0 when h = 0.  This is ROUGE.pl's P R / (0.5 P + 0.5 R) (alpha 0.5)
+ *   without its 5-decimal rounding.  Counting is integer, so the result does not depend on the launch.
+ * Errors: NULL arguments, n_ref < 1, rows_per_ref < 1, n != n_ref * rows_per_ref, a cap < 1,
+ * ref_cap + cand_cap > NATS_ROUGE_MAX_CAP. */
+int nats_rouge_f(nats_ctx_t* ctx, void* stream, const int32_t* cand, int cand_cap, const int32_t* cand_len, int n,
+                 const int32_t* ref, int ref_cap, const int32_t* ref_len, int n_ref, int rows_per_ref, float* out);
 
 /* ---------------------------------------------------------------- diagnostics ------------------- */
 /* The library's internal GEMM engine, exposed for the parity tests: C = op(A).op(B) (+bias) (+C), row-major,

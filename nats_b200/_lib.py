@@ -11,6 +11,7 @@ HEADER_PATH = os.path.join(os.path.dirname(_HERE), 'include', 'nats_b200.h')
 
 NUM_PARAMS = 43
 GRAD_TAIL = 32
+ROUGE_MAX_CAP = 4096      # NATS_ROUGE_MAX_CAP
 
 
 class Dims(Structure):
@@ -71,6 +72,10 @@ SIGNATURES = {
                                      c_float, _P]),
     'nats_train_bwd_finish': (c_int, [c_void_p, _P, POINTER(Dims), _P, _P, _P, _P, _P, c_int, c_int, c_int, _P, c_int64,
                                       c_float, _P]),
+    'nats_train_bwd_weighted': (c_int, [c_void_p, _P, POINTER(Dims), _P, _P, _P, _P, _P, c_int, c_int, c_int, _P, c_int64,
+                                        c_float, _P, _P]),
+    'nats_train_bwd_begin_weighted': (c_int, [c_void_p, _P, POINTER(Dims), _P, _P, _P, _P, _P, c_int, c_int, c_int, _P,
+                                              c_int64, c_float, _P, _P]),
     'nats_encoder_fwd': (c_int, [c_void_p, _P, POINTER(Dims), _P, _P, _P, c_int, c_int, c_int, _P, c_int64]),
     'nats_decoder_scan_fwd': (c_int, [c_void_p, _P, POINTER(Dims), _P, _P, _P, _P, c_int, c_int, c_int, _P, c_int64]),
     'nats_readout_nll_fwd': (c_int, [c_void_p, _P, POINTER(Dims), _P, _P, _P, c_int, c_int, c_int, _P, c_int64, _P]),
@@ -100,6 +105,7 @@ SIGNATURES = {
     'nats_beam_step': (c_int, [c_void_p, _P, POINTER(Dims), POINTER(BeamStep), c_int]),
     'nats_beam_step_many': (c_int, [c_void_p, _P, POINTER(Dims), POINTER(BeamStepMany), c_int]),
     'nats_sample_step_many': (c_int, [c_void_p, _P, POINTER(Dims), POINTER(SampleStepMany), c_int]),
+    'nats_rouge_f': (c_int, [c_void_p, _P, _P, c_int, _P, c_int, _P, c_int, _P, c_int, c_int, _P]),
     'nats_debug_gemm': (c_int, [c_void_p, _P, c_int, c_int, c_int, c_int, c_int, c_int, _P, c_int, _P, c_int, _P, c_int,
                                 _P, c_int, c_int, c_int, c_int64, c_int64, c_int64]),
     'nats_profile_enable': (c_int, [c_void_p, c_int]),

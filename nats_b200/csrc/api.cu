@@ -31,7 +31,7 @@ const char* kNames[K_COUNT] = {
     "gemm_mid_tt", "gemm_smallm_nn", "gemm_smallm_nt", "gemm_smallm_tn", "gemm_smallm_tt", "gru_gates_fwd",
     "gru_gates_bwd", "att_scores", "att_context", "att_bwd_ctx", "att_bwd_dalpha", "att_bwd_softmax", "nll_rows",
     "dlogits", "softmax_sample", "colsum", "reduce_splits", "embedding", "elementwise", "optimizer", "beam",
-    "memset", "tc_gemm_3xtf32", "tc_gemm_3xtf32_skinny", "enc_tc_fwd", "enc_tc_bwd", "sample"};
+    "memset", "tc_gemm_3xtf32", "tc_gemm_3xtf32_skinny", "enc_tc_fwd", "enc_tc_bwd", "sample", "rouge"};
 }  // namespace
 const char* kclass_name(int cls) { return (cls >= 0 && cls < K_COUNT) ? kNames[cls] : "?"; }
 bool prof_enabled() { return g_prof.on; }
@@ -75,7 +75,7 @@ struct ViewDef { const char* name; int64_t off; int rows, cols, ld, ndim; };
 extern "C" {
 
 const char* nats_last_error(void) { return g_err; }
-int nats_version(void) { return 103; }
+int nats_version(void) { return 104; }
 
 int nats_ctx_create(int device, nats_ctx_t** out) {
     NATS_REQUIRE(out != nullptr, "out");
@@ -262,7 +262,7 @@ int nats_readout_nll_bwd(nats_ctx_t* ctx, void* stream, const nats_dims_t* dims,
                          const int64_t* y, const float* y_mask, int Tx, int Ty, int B, void* ws, int64_t ws_bytes,
                          float scale, float* grads) {
     NATS_TRAIN_PROLOGUE();
-    return train_readout_bwd(ctx, st, *dims, params, y, y_mask, Ty, B, w, scale, grads);
+    return train_readout_bwd(ctx, st, *dims, params, y, y_mask, Ty, B, w, scale, nullptr, grads);
 }
 
 int nats_decoder_scan_bwd(nats_ctx_t* ctx, void* stream, const nats_dims_t* dims, const float* params,
@@ -295,17 +295,38 @@ int64_t nats_grad_split(const nats_dims_t* dims) {
     return param_offsets(*dims).ff_state_W;      // [Wemb | encoder | encoder_r] come first in the flat layout
 }
 
-int nats_train_bwd_begin(nats_ctx_t* ctx, void* stream, const nats_dims_t* dims, const float* params, const int64_t* x,
-                         const float* x_mask, const int64_t* y, const float* y_mask, int Tx, int Ty, int B, void* ws,
-                         int64_t ws_bytes, float scale, float* grads) {
+}  // extern "C"
+
+namespace {
+// the first half of the backward; weight [B] (NULL = ones) scales sample b's cost, and with it every gradient, through
+// d logits and the cost tail alone: the rest of the backward is linear in d logits
+int train_bwd_begin(nats_ctx_t* ctx, void* stream, const nats_dims_t* dims, const float* params, const int64_t* x,
+                    const float* x_mask, const int64_t* y, const float* y_mask, int Tx, int Ty, int B, void* ws,
+                    int64_t ws_bytes, float scale, const float* weight, float* grads) {
     NATS_TRAIN_PROLOGUE();
     NATS_REQUIRE(x && x_mask && y && y_mask && grads && params, "null argument");
     const ParamOff o = param_offsets(*dims);
     NATS_CUDA_OK(memset_async(st, grads, 0, (size_t)(o.total + NATS_GRAD_TAIL) * sizeof(float)));
-    NATS_TRY(cost_reduce(st, w.rowcost, Ty, B, nullptr, scale, grads + o.total));
-    NATS_TRY(train_readout_bwd(ctx, st, *dims, params, y, y_mask, Ty, B, w, scale, grads));
+    NATS_TRY(cost_reduce(st, w.rowcost, Ty, B, nullptr, scale, weight, grads + o.total));
+    NATS_TRY(train_readout_bwd(ctx, st, *dims, params, y, y_mask, Ty, B, w, scale, weight, grads));
     NATS_TRY(train_decoder_bwd(ctx, st, *dims, params, y, x_mask, y_mask, Tx, Ty, B, w, grads));
     return 0;
+}
+}  // namespace
+
+extern "C" {
+
+int nats_train_bwd_begin(nats_ctx_t* ctx, void* stream, const nats_dims_t* dims, const float* params, const int64_t* x,
+                         const float* x_mask, const int64_t* y, const float* y_mask, int Tx, int Ty, int B, void* ws,
+                         int64_t ws_bytes, float scale, float* grads) {
+    return train_bwd_begin(ctx, stream, dims, params, x, x_mask, y, y_mask, Tx, Ty, B, ws, ws_bytes, scale, nullptr, grads);
+}
+
+int nats_train_bwd_begin_weighted(nats_ctx_t* ctx, void* stream, const nats_dims_t* dims, const float* params,
+                                  const int64_t* x, const float* x_mask, const int64_t* y, const float* y_mask, int Tx, int Ty,
+                                  int B, void* ws, int64_t ws_bytes, float scale, const float* weight, float* grads) {
+    NATS_REQUIRE(weight != nullptr, "weight (the unweighted step is nats_train_bwd_begin)");
+    return train_bwd_begin(ctx, stream, dims, params, x, x_mask, y, y_mask, Tx, Ty, B, ws, ws_bytes, scale, weight, grads);
 }
 
 int nats_train_bwd_finish(nats_ctx_t* ctx, void* stream, const nats_dims_t* dims, const float* params, const int64_t* x,
@@ -321,6 +342,14 @@ int nats_train_bwd(nats_ctx_t* ctx, void* stream, const nats_dims_t* dims, const
                    const float* x_mask, const int64_t* y, const float* y_mask, int Tx, int Ty, int B, void* ws,
                    int64_t ws_bytes, float scale, float* grads) {
     NATS_TRY(nats_train_bwd_begin(ctx, stream, dims, params, x, x_mask, y, y_mask, Tx, Ty, B, ws, ws_bytes, scale, grads));
+    return nats_train_bwd_finish(ctx, stream, dims, params, x, x_mask, y, y_mask, Tx, Ty, B, ws, ws_bytes, scale, grads);
+}
+
+int nats_train_bwd_weighted(nats_ctx_t* ctx, void* stream, const nats_dims_t* dims, const float* params, const int64_t* x,
+                            const float* x_mask, const int64_t* y, const float* y_mask, int Tx, int Ty, int B, void* ws,
+                            int64_t ws_bytes, float scale, const float* weight, float* grads) {
+    NATS_TRY(nats_train_bwd_begin_weighted(ctx, stream, dims, params, x, x_mask, y, y_mask, Tx, Ty, B, ws, ws_bytes, scale,
+                                           weight, grads));
     return nats_train_bwd_finish(ctx, stream, dims, params, x, x_mask, y, y_mask, Tx, Ty, B, ws, ws_bytes, scale, grads);
 }
 
@@ -673,5 +702,16 @@ int nats_sample_step_many(nats_ctx_t* ctx, void* stream, const nats_dims_t* dims
     return sample_step_group(ctx, reinterpret_cast<cudaStream_t>(stream), dims, a, step);
 }
 
+// ------------------------------------------------------------------------------------------ rewards
+int nats_rouge_f(nats_ctx_t* ctx, void* stream, const int32_t* cand, int cand_cap, const int32_t* cand_len, int n,
+                 const int32_t* ref, int ref_cap, const int32_t* ref_len, int n_ref, int rows_per_ref, float* out) {
+    NATS_REQUIRE(ctx && cand && cand_len && ref && ref_len && out, "null argument");
+    NATS_REQUIRE(n_ref >= 1 && rows_per_ref >= 1 && (long long)n_ref * rows_per_ref == (long long)n,
+                 "n must equal n_ref * rows_per_ref (both >= 1)");
+    NATS_REQUIRE(cand_cap >= 1 && ref_cap >= 1 && (long long)cand_cap + ref_cap <= NATS_ROUGE_MAX_CAP,
+                 "caps: >= 1 each, ref_cap + cand_cap <= NATS_ROUGE_MAX_CAP");
+    return rouge_f(reinterpret_cast<cudaStream_t>(stream), cand, cand_cap, cand_len, n, ref, ref_cap, ref_len, rows_per_ref,
+                   out);
+}
 
 }  // extern "C"

@@ -16,7 +16,7 @@ PKG = os.path.dirname(HERE)
 ROOT = os.path.dirname(PKG)
 OUT = os.path.join(PKG, 'libnats_b200.so')
 OBJ = os.path.join(HERE, 'build')
-SOURCES = ['gemm.cu', 'tc_gemm.cu', 'tma_gemm.cu', 'enc_tc.cu', 'ops_elem.cu', 'ops_att.cu', 'ops_readout.cu', 'ops_optim.cu', 'ops_beam.cu',
+SOURCES = ['gemm.cu', 'tc_gemm.cu', 'tma_gemm.cu', 'enc_tc.cu', 'ops_elem.cu', 'ops_att.cu', 'ops_readout.cu', 'ops_optim.cu', 'ops_beam.cu', 'ops_rouge.cu',
            'model_fwd.cu', 'model_bwd.cu', 'api.cu']
 HEADERS = ['common.cuh', 'prof.cuh', 'tc_common.cuh', 'gemm.cuh', 'gates.cuh', 'ops.cuh', 'workspace.cuh', 'model.cuh',
            os.path.join(ROOT, 'include', 'nats_b200.h')]

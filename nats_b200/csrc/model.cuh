@@ -52,7 +52,7 @@ int train_readout_fwd(const nats_ctx* ctx, cudaStream_t st, const nats_dims_t& d
                       const int64_t* y, const float* y_mask, int Ty, int B, const TrainWS& w, float* cost);
 int train_readout_bwd(const nats_ctx* ctx, cudaStream_t st, const nats_dims_t& d, const float* params,
                       const int64_t* y, const float* y_mask, int Ty, int B, const TrainWS& w, float scale,
-                      float* grads);
+                      const float* weight /* [B] or NULL */, float* grads);
 int train_decoder_bwd(const nats_ctx* ctx, cudaStream_t st, const nats_dims_t& d, const float* params,
                       const int64_t* y, const float* x_mask, const float* y_mask, int Tx, int Ty, int B,
                       const TrainWS& w, float* grads);

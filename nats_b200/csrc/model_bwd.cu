@@ -19,11 +19,11 @@ inline int ga(const nats_ctx* ctx, cudaStream_t st, const TrainWS& w, GemmProble
 // ------------------------------------------------------------------ readout (nats.py:753-770)
 int train_readout_bwd(const nats_ctx* ctx, cudaStream_t st, const nats_dims_t& d, const float* params,
                       const int64_t* y, const float* y_mask, int Ty, int B, const TrainWS& w, float scale,
-                      float* G) {
+                      const float* weight, float* G) {
     const ParamOff o = param_offsets(d);
     const int W = d.dim_word, D = d.dim, V = d.n_words, C = 2 * D;
     const int YB = Ty * B;
-    NATS_TRY(dlogits_inplace(st, w.logits, YB, V, y, y_mask, w.lse, scale));
+    NATS_TRY(dlogits_inplace(st, w.logits, YB, V, y, y_mask, w.lse, scale, weight, B));
     // ff_logit: dW = L^T dlogits, db = colsum, dL = dlogits W^T
     NATS_TRY(ga(ctx, st, w, gemm_problem(w.L, W, w.logits, V, G + o.logit_W, V, W, V, YB), true, false));
     NATS_TRY(colsum(st, w.logits, YB, V, V, G + o.logit_b, 0, w.red_scratch));

@@ -242,7 +242,7 @@ int train_readout_fwd(const nats_ctx* ctx, cudaStream_t st, const nats_dims_t& d
     p.bias = params + o.logit_b;
     NATS_TRY(gemm_auto(ctx, st, p, false, false, w.gemm_scratch, w.gemm_scratch_floats));
     NATS_TRY(nll_rows(st, w.logits, YB, V, y, y_mask, w.lse, w.rowcost));
-    NATS_TRY(cost_reduce(st, w.rowcost, Ty, B, cost, 1.f, nullptr));
+    NATS_TRY(cost_reduce(st, w.rowcost, Ty, B, cost, 1.f, nullptr, nullptr));
     return 0;
 }
 

@@ -113,8 +113,9 @@ int colsum3(cudaStream_t st, const float* X, long long K, int N, int ld, float* 
 // out[n] (+)= sum_k X[k*ld+n] * Y[k*ld+n]        (d U_con, d W_con)
 int colsum_prod(cudaStream_t st, const float* X, const float* Y, long long K, int N, int ld, float* out,
                 int accumulate, float* scratch);
-// cost[b] = sum_t rowcost[t*B+b];   *total (device scalar) = scale * sum_b cost[b]
-int cost_reduce(cudaStream_t st, const float* rowcost, int Ty, int B, float* cost, float scale, float* total);
+// cost[b] = sum_t rowcost[t*B+b];   *total (device scalar) = scale * sum_b weight[b] * cost[b]   (weight NULL = ones)
+int cost_reduce(cudaStream_t st, const float* rowcost, int Ty, int B, float* cost, float scale, const float* weight,
+                float* total);
 
 // ------------------------------------------------------------------ attention + distraction (nats.py:527-546, 569-570)
 struct AttFwd {
@@ -168,9 +169,9 @@ int attention_bwd(const nats_ctx* ctx, cudaStream_t st, const AttBwd& a);
 // per row r: lse[r] = logsumexp(logits[r,:]); rowcost[r] = (lse[r] - logits[r, y[r]]) * ymask[r]
 int nll_rows(cudaStream_t st, const float* logits, int rows, int V, const int64_t* y, const float* ymask,
              float* lse, float* rowcost);
-// logits[r,v] <- (exp(logits[r,v]-lse[r]) - [v==y[r]]) * ymask[r] * scale
+// logits[r,v] <- (exp(logits[r,v]-lse[r]) - [v==y[r]]) * ymask[r] * scale (* weight[r % B] unless weight is NULL)
 int dlogits_inplace(cudaStream_t st, float* logits, int rows, int V, const int64_t* y, const float* ymask,
-                    const float* lse, float scale);
+                    const float* lse, float scale, const float* weight, int B);
 // probs[r,:] = softmax(logits[r,:]); sample[r] ~ multinomial(probs[r,:]) (counter-based RNG)
 int softmax_sample_rows(cudaStream_t st, const float* logits, int rows, int V, float* probs, int64_t* sample,
                         uint64_t seed, uint64_t step);
@@ -224,5 +225,11 @@ int beam_advance(cudaStream_t st, const int32_t* parents, const int32_t* fin_par
                  float* acc_ctx_n, const float* acc_alpha_o, float* acc_alpha_n, const float* cur_alpha, const float* cur_ctx,
                  const float* cur_state, const float* hist_alpha_src, float* hist_alpha_dst, const float* hist_ctx_src,
                  float* hist_ctx_dst, const float* hist_state_src, float* hist_state_dst, float* out_alpha);
+
+// ------------------------------------------------------------------ ROUGE of token-id rows (ops_rouge.cu)
+constexpr int kRougeMaxCap = NATS_ROUGE_MAX_CAP;   // ref_cap + cand_cap: both rows and the LCS diagonals in shared memory
+// out [3, n]: ROUGE-1, ROUGE-2 and ROUGE-L F of candidate row r against reference row r / rows_per_ref (nats_rouge_f)
+int rouge_f(cudaStream_t st, const int32_t* cand, int cand_cap, const int32_t* cand_len, int n, const int32_t* ref,
+            int ref_cap, const int32_t* ref_len, int rows_per_ref, float* out);
 
 }  // namespace nats

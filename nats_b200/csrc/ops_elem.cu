@@ -191,14 +191,14 @@ __global__ void colsum_stage2(const float* __restrict__ part, int ks, int N, flo
 }
 
 __global__ void cost_reduce_kernel(const float* __restrict__ rowcost, int Ty, int B, float* __restrict__ cost,
-                                   float scale, float* __restrict__ total) {
+                                   float scale, const float* __restrict__ weight, float* __restrict__ total) {
     __shared__ float red[32];
     float acc = 0.f;
     for (int b = threadIdx.x; b < B; b += blockDim.x) {
         float s = 0.f;
         for (int t = 0; t < Ty; ++t) s += rowcost[(long long)t * B + b];
         if (cost) cost[b] = s;
-        acc += s;
+        acc += weight ? weight[b] * s : s;
     }
     acc = block_sum(acc, red);
     if (threadIdx.x == 0 && total) *total = acc * scale;
@@ -317,9 +317,10 @@ int colsum_prod(cudaStream_t st, const float* X, const float* Y, long long K, in
                 int accumulate, float* scratch) {
     return colsum_impl(st, X, Y, K, N, ld, out, accumulate, scratch);
 }
-int cost_reduce(cudaStream_t st, const float* rowcost, int Ty, int B, float* cost, float scale, float* total) {
+int cost_reduce(cudaStream_t st, const float* rowcost, int Ty, int B, float* cost, float scale, const float* weight,
+                float* total) {
     ProfScope ps(st, K_ELEMWISE);
-    cost_reduce_kernel<<<1, 256, 0, st>>>(rowcost, Ty, B, cost, scale, total);
+    cost_reduce_kernel<<<1, 256, 0, st>>>(rowcost, Ty, B, cost, scale, weight, total);
     NATS_LAUNCH_OK();
     return 0;
 }

@@ -32,11 +32,13 @@ __global__ void __launch_bounds__(kRowThreads) nll_rows_kernel(const float* __re
 }
 
 __global__ void dlogits_kernel(float* __restrict__ logits, int rows, int V, const int64_t* __restrict__ y,
-                               const float* __restrict__ ymask, const float* __restrict__ lse, float scale) {
+                               const float* __restrict__ ymask, const float* __restrict__ lse, float scale,
+                               const float* __restrict__ weight, int B) {
     // rows on grid.x (2^31 - 1 blocks), vocabulary chunks on grid.y: rows = Ty*B exceeds the 65535 limit of grid.y for
     // large batches (e.g. batch 160 at maxlen 500)
     const int r = blockIdx.x;
-    const float w = (ymask ? ymask[r] : 1.f) * scale;
+    float w = (ymask ? ymask[r] : 1.f) * scale;
+    if (weight) w *= weight[r % B];                              // row r = t*B + b carries sample b's weight
     const float l = lse[r];
     const long long id = y[r];
     float* row = logits + (long long)r * V;
@@ -641,14 +643,14 @@ int nll_rows(cudaStream_t st, const float* logits, int rows, int V, const int64_
     return 0;
 }
 int dlogits_inplace(cudaStream_t st, float* logits, int rows, int V, const int64_t* y, const float* ymask,
-                    const float* lse, float scale) {
+                    const float* lse, float scale, const float* weight, int B) {
     if (rows == 0) return 0;
     int gy = cdiv(V, 256 * 4);
     if (gy < 1) gy = 1;
     if (gy > 65535) gy = 65535;
     dim3 grid(rows, gy);
     ProfScope ps(st, K_DLOGITS, 0.0, 8.0 * rows * V);
-    dlogits_kernel<<<grid, 256, 0, st>>>(logits, rows, V, y, ymask, lse, scale);
+    dlogits_kernel<<<grid, 256, 0, st>>>(logits, rows, V, y, ymask, lse, scale, weight, B);
     NATS_LAUNCH_OK();
     return 0;
 }

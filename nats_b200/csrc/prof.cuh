@@ -29,6 +29,7 @@ enum KClass {
     K_ENC_PERSIST_FWD,   // persistent weight-stationary wgmma bidirectional encoder recurrence (one launch per pass)
     K_ENC_PERSIST_BWD,
     K_SAMPLE,            // filtered sampling: bans, draw and bookkeeping of nats_sample_step_many
+    K_ROUGE,             // ROUGE-1 / 2 / L F of token-id rows (nats_rouge_f)
     K_COUNT
 };
 

@@ -329,7 +329,8 @@ def _bucket(n, q):
 
 class _Arena(object):
     """Storage shared by every plan of a ModelGraph: ONE workspace sized for the largest shape seen, one packed device
-    input buffer (x | y | x_mask | y_mask) and its pinned host mirror -> one H2D copy per step.  Plans are views; when the
+    input buffer (x | y | x_mask | y_mask, then the per-sample weights of a weighted step) and its pinned host mirror -> one
+    H2D copy per step.  Plans are views; when the
     arena has to grow (a larger shape than any before) every captured CUDA graph is dropped with the old addresses."""
 
     def __init__(self, model):
@@ -355,7 +356,7 @@ class _Arena(object):
         need_ws = int(eng.lib.nats_train_workspace_bytes(ctypes.byref(self.model.dims), Tx, Ty, B))
         if need_ws <= 0:
             raise NatsB200Error('nats_train_workspace_bytes failed')
-        need_in = self.input_layout(Tx, Ty, B)[4]
+        need_in = self.input_layout(Tx, Ty, B)[4] + B * 4       # + the weights [B] of a weighted step
         grown = False
         if need_ws > self.ws_bytes:
             self.ws = None
@@ -391,23 +392,33 @@ class _TrainPlan(object):
         self.x, self.y, self.xm, self.ym = views(arena.inp)
         self.hx, self.hy, self.hxm, self.hym = [t.numpy() for t in views(arena.pin)]      # numpy views of the pinned mirror
         self.dev_in, self.pin_in = arena.inp[:end], arena.pin[:end]
+        self.w = arena.inp[end:end + B * 4].view(torch.float32)                          # weights of a weighted step
+        self.hw = arena.pin[end:end + B * 4].view(torch.float32).numpy()
+        self.dev_in_w, self.pin_in_w = arena.inp[:end + B * 4], arena.pin[:end + B * 4]
         self.cost = torch.zeros((B,), dtype=torch.float32, device=model.engine.device)
         self.graph_fwd = None      # forward only (f_log_probs)
         self.graph_fb = None       # forward + first half of the backward (data-parallel)
         self.graph_fb2 = None      # second half of the backward (encoder), overlapped with the first all-reduce
         self.graph_post = None     # L2 / clip / optimiser accumulators
         self.graph_step = None     # single GPU: forward + backward + post in one graph
+        self.graph_fb_w = None     # the weighted twins of graph_fb / graph_step (graph_fb2 and graph_post serve both)
+        self.graph_step_w = None
         self.uses = 0
 
-    def stage(self, x, x_mask, y, y_mask):
-        """host arrays (any shape <= the plan's: the rest is zero padding, masked out) -> pinned mirror -> ONE H2D copy"""
+    def stage(self, x, x_mask, y, y_mask, weights=None):
+        """host arrays (any shape <= the plan's: the rest is zero padding, masked out) -> pinned mirror -> ONE H2D copy;
+        weights [B] (a weighted step) travel in the same copy"""
         Tx, Ty, B = self.shape
         for dst, src in ((self.hx, x), (self.hxm, x_mask), (self.hy, y), (self.hym, y_mask)):
             t = src.shape[0]
             dst[:t] = src
             if t < dst.shape[0]:
                 dst[t:] = 0
-        self.dev_in.copy_(self.pin_in, non_blocking=True)
+        if weights is None:
+            self.dev_in.copy_(self.pin_in, non_blocking=True)
+        else:
+            self.hw[:] = weights
+            self.dev_in_w.copy_(self.pin_in_w, non_blocking=True)
 
     def h2d_bytes(self):
         return int(self.in_bytes)
@@ -512,11 +523,17 @@ class ModelGraph(object):
         _lib.check(eng.lib.nats_train_fwd(*(self._train_args(p) + (_ptr(p.cost),))), 'nats_train_fwd')
         eng.launches += 1
 
-    def enqueue_bwd(self, p, scale, part=0):
-        """part 0: whole backward; 1: readout + decoder (grads[split:] final); 2: encoder (grads[:split] final)"""
+    def enqueue_bwd(self, p, scale, part=0, weighted=False):
+        """part 0: whole backward; 1: readout + decoder (grads[split:] final); 2: encoder (grads[:split] final).
+        weighted: parts 0 and 1 scale sample b's cost by the staged weight p.w[b]"""
         eng = self.engine
-        fn = (eng.lib.nats_train_bwd, eng.lib.nats_train_bwd_begin, eng.lib.nats_train_bwd_finish)[part]
-        _lib.check(fn(*(self._train_args(p) + (ctypes.c_float(scale), _ptr(self.grads)))), 'nats_train_bwd')
+        if weighted and part != 2:
+            fn = (eng.lib.nats_train_bwd_weighted, eng.lib.nats_train_bwd_begin_weighted)[part]
+            args = self._train_args(p) + (ctypes.c_float(scale), _ptr(p.w), _ptr(self.grads))
+        else:
+            fn = (eng.lib.nats_train_bwd, eng.lib.nats_train_bwd_begin, eng.lib.nats_train_bwd_finish)[part]
+            args = self._train_args(p) + (ctypes.c_float(scale), _ptr(self.grads))
+        _lib.check(fn(*args), 'nats_train_bwd')
         eng.launches += 1
 
     def enqueue_clip(self):
@@ -586,11 +603,13 @@ class ModelGraph(object):
                 return hb[0] + (self.decay_c * hb[1] if self.decay_c > 0. else 0.0)
         return LazyCost(_B(), ev)
 
-    def grad_step(self, x, x_mask, y, y_mask, after_grads, global_batch=None):
+    def grad_step(self, x, x_mask, y, y_mask, after_grads, global_batch=None, weights=None):
         """forward + backward (+ allreduce) + L2/clip + `after_grads()` (the optimiser's accumulator update);
         returns the scalar cost like f_grad_shared (nats.py:1160).  `global_batch`: number of sentence pairs of the
         whole data-parallel step (default: local batch x world size).  x = None: this rank's shard is empty; it only
-        contributes zeros to the all-reduce."""
+        contributes zeros to the all-reduce.  weights [B] (an addition beyond the reference): the step differentiates
+        scale * sum_b weights[b] * cost_b instead, and returns that sum (nats_train_bwd_weighted); None is the
+        reference's step."""
         torch = self.engine.torch
         world = self.world
         if x is None:
@@ -601,9 +620,14 @@ class ModelGraph(object):
             after_grads()
             c = self._read_cost()
             return c if self.lazy_cost else c.value()
-        p = self.plan(x.shape[0], y.shape[0], x.shape[1])
-        p.stage(x, x_mask, y, y_mask)
         B = x.shape[1]
+        wt = weights is not None
+        if wt:
+            weights = numpy.asarray(weights, dtype='float32').reshape(-1)
+            if weights.shape[0] != B:
+                raise ValueError('weights: %d values for a batch of %d' % (weights.shape[0], B))
+        p = self.plan(x.shape[0], y.shape[0], x.shape[1])
+        p.stage(x, x_mask, y, y_mask, weights)
         scale = parallel.grad_scale(B, world, global_batch)   # d mean(cost) over the GLOBAL batch (nats.py:1323)
 
         def post():
@@ -611,9 +635,11 @@ class ModelGraph(object):
             after_grads()
 
         if world == 1:
-            self._run(p, 'graph_step', lambda: (self.enqueue_fwd(p), self.enqueue_bwd(p, scale), post()))
+            self._run(p, 'graph_step_w' if wt else 'graph_step',
+                      lambda: (self.enqueue_fwd(p), self.enqueue_bwd(p, scale, weighted=wt), post()))
         elif not self.overlap_allreduce:
-            self._run(p, 'graph_fb', lambda: (self.enqueue_fwd(p), self.enqueue_bwd(p, scale)))
+            self._run(p, 'graph_fb_w' if wt else 'graph_fb',
+                      lambda: (self.enqueue_fwd(p), self.enqueue_bwd(p, scale, weighted=wt)))
             parallel.allreduce_flat(self.grads)               # ONE collective: gradients + cost tail
             self._run(p, 'graph_post', post)
         else:
@@ -626,7 +652,8 @@ class ModelGraph(object):
                 self._pg_side_tried = True
                 self._pg_side = parallel.side_group(int(os.environ.get('NATS_NCCL_SIDE_CTAS', '4')))
             main = torch.cuda.current_stream(self.engine.device)
-            self._run(p, 'graph_fb', lambda: (self.enqueue_fwd(p), self.enqueue_bwd(p, scale, 1)))
+            self._run(p, 'graph_fb_w' if wt else 'graph_fb',
+                      lambda: (self.enqueue_fwd(p), self.enqueue_bwd(p, scale, 1, weighted=wt)))
             self._side.wait_stream(main)
             with torch.cuda.stream(self._side):
                 w1 = parallel.allreduce_flat(self.grads[self.split:], async_op=True, group=self._pg_side)
@@ -683,8 +710,8 @@ def adadelta(lr, tparams, grads, inp, cost, epsilon=1e-6, rho=0.95):
                    'nats_adadelta_grad_shared')
         eng.launches += 1
 
-    def f_grad_shared(x, x_mask, y, y_mask, global_batch=None):
-        return graph.grad_step(x, x_mask, y, y_mask, accum, global_batch=global_batch)
+    def f_grad_shared(x, x_mask, y, y_mask, global_batch=None, weights=None):
+        return graph.grad_step(x, x_mask, y, y_mask, accum, global_batch=global_batch, weights=weights)
 
     def f_update(lr_value=None):
         _lib.check(eng.lib.nats_adadelta_update(eng.ctx, eng.stream(), n, _ptr(tparams.flat), _ptr(graph.grads),
@@ -705,8 +732,8 @@ def adam(lr, tparams, grads, inp, cost):
     n = tparams.total
     step = numpy.zeros(1, dtype='int64')
 
-    def f_grad_shared(x, x_mask, y, y_mask, global_batch=None):
-        return graph.grad_step(x, x_mask, y, y_mask, lambda: None, global_batch=global_batch)
+    def f_grad_shared(x, x_mask, y, y_mask, global_batch=None, weights=None):
+        return graph.grad_step(x, x_mask, y, y_mask, lambda: None, global_batch=global_batch, weights=weights)
 
     def f_update(lr_value=None):
         _lib.check(eng.lib.nats_adam_update(eng.ctx, eng.stream(), n, _ptr(tparams.flat), _ptr(graph.grads),
@@ -730,8 +757,8 @@ def rmsprop(lr, tparams, grads, inp, cost):
                                                     _ptr(rg2)), 'nats_rmsprop_grad_shared')
         eng.launches += 1
 
-    def f_grad_shared(x, x_mask, y, y_mask, global_batch=None):
-        return graph.grad_step(x, x_mask, y, y_mask, accum, global_batch=global_batch)
+    def f_grad_shared(x, x_mask, y, y_mask, global_batch=None, weights=None):
+        return graph.grad_step(x, x_mask, y, y_mask, accum, global_batch=global_batch, weights=weights)
 
     def f_update(lr_value=None):
         _lib.check(eng.lib.nats_rmsprop_update(eng.ctx, eng.stream(), n, _ptr(tparams.flat), _ptr(graph.grads),
@@ -748,8 +775,8 @@ def sgd(lr, tparams, grads, inp, cost):
     provided here with the common 5-argument form: p <- p - lr * g."""
     graph = grads
 
-    def f_grad_shared(x, x_mask, y, y_mask, global_batch=None):
-        return graph.grad_step(x, x_mask, y, y_mask, lambda: None, global_batch=global_batch)
+    def f_grad_shared(x, x_mask, y, y_mask, global_batch=None, weights=None):
+        return graph.grad_step(x, x_mask, y, y_mask, lambda: None, global_batch=global_batch, weights=weights)
 
     def f_update(lr_value):
         tparams.flat.add_(graph.grads[:tparams.total], alpha=-float(lr_value))
@@ -1621,6 +1648,137 @@ def sample_many(tparams, f_init, f_next, xs, options, n_samples=5, maxlen=30, te
                                                                         (index_base + first) * R, slot, stream))
 
 
+def _id_rows(rows, what):
+    """list of id lists -> (int32 [len(rows), cap] zero padded, int32 lengths, cap >= 1), checked on the host"""
+    if isinstance(rows, (str, bytes)) or not hasattr(rows, '__len__'):
+        raise ValueError('%s must be a list of id lists' % what)
+    seqs = []
+    for s in rows:
+        a = numpy.asarray(s if hasattr(s, '__len__') else [s])
+        if a.ndim != 1 or (a.size and a.dtype.kind not in 'iu'):
+            raise ValueError('%s: every row must be a flat list of integer ids' % what)
+        if a.size and (a.min() < -2 ** 31 or a.max() >= 2 ** 31):
+            raise ValueError('%s: ids must fit in int32' % what)
+        seqs.append(a)
+    cap = max([1] + [a.size for a in seqs])
+    ids = numpy.zeros((len(seqs), cap), dtype='int32')
+    for i, a in enumerate(seqs):
+        ids[i, :a.size] = a
+    return ids, numpy.array([a.size for a in seqs], dtype='int32'), cap
+
+
+def rouge_f(cands, refs, rows_per_ref=1):
+    """ROUGE-1, ROUGE-2 and ROUGE-L F of token-id sequences on the device (an addition beyond the reference; the reward of
+    self-critical training) -> numpy float32 [3, n], n = len(cands): row r is scored against refs[r // rows_per_ref].
+    A sequence's words end at its first 0 (EOS); UNK (1) matches nothing.  The values are those of evaluate.rouge_n(1),
+    rouge_n(2) and rouge_l on the space-joined words (UNKs renamed apart) without ROUGE.pl's 5-decimal rounding: exactly
+    (float)(2 hits) / (float)(m + c) (nats_rouge_f, include/nats_b200.h).  The ids travel in one host-to-device copy.
+    Invalid arguments raise ValueError before anything is launched."""
+    if int(rows_per_ref) != rows_per_ref or rows_per_ref < 1:
+        raise ValueError('rows_per_ref must be an integer >= 1, got %r' % (rows_per_ref,))
+    rows_per_ref = int(rows_per_ref)
+    c_ids, c_len, c_cap = _id_rows(cands, 'cands')
+    r_ids, r_len, r_cap = _id_rows(refs, 'refs')
+    n, n_ref = c_ids.shape[0], r_ids.shape[0]
+    if n_ref < 1 or n != n_ref * rows_per_ref:
+        raise ValueError('%d candidates for %d references x %d rows each' % (n, n_ref, rows_per_ref))
+    if c_cap + r_cap > _lib.ROUGE_MAX_CAP:
+        raise ValueError('longest candidate + longest reference = %d ids; at most %d' % (c_cap + r_cap, _lib.ROUGE_MAX_CAP))
+    eng = get_engine()
+    torch = eng.torch
+    parts = (c_ids.ravel(), c_len, r_ids.ravel(), r_len)
+    offs = numpy.cumsum([0] + [a.size for a in parts])
+    pin = torch.empty(int(offs[-1]), dtype=torch.int32).pin_memory()
+    hp = pin.numpy()
+    for o, a in zip(offs, parts):
+        hp[o:o + a.size] = a
+    dev = pin.to(eng.device, non_blocking=True)
+    out = torch.empty((3, n), dtype=torch.float32, device=eng.device)
+    ptr = lambda i: ctypes.c_void_p(dev.data_ptr() + 4 * int(offs[i]))
+    _lib.check(eng.lib.nats_rouge_f(eng.ctx, eng.stream(), ptr(0), c_cap, ptr(1), n, ptr(2), r_cap, ptr(3), n_ref,
+                                    rows_per_ref, _ptr(out)), 'nats_rouge_f')
+    eng.launches += 1
+    return out.cpu().numpy()
+
+
+def scst_batch(seqs_x, seqs_y, samples, rewards, baselines, gamma):
+    """One self-critical training batch (an addition beyond the reference) for B sources with R samples each -> (x, x_mask,
+    y, y_mask, weights), columns in this order:
+      * the B ground-truth pairs (seqs_x[b], seqs_y[b]) with weight 1 - gamma (left out when gamma = 1);
+      * the B*R sampled pairs (seqs_x[b], sample b*R + j) with weight gamma * (rewards[b*R + j] - baselines[b]) / R.
+    A sample is a drawn word list as sample_many returns it: ending with 0 (EOS) when the model ended it, without when
+    maxlen cut it.  Its target is its words without the EOS; the implicit EOS row of prepare_data keeps mask 1 only for
+    a sample that ended with EOS, so a cut sample is not trained towards an EOS it never drew.  Summed with scale
+    1 / B_global, the weighted costs are (1/B_global) sum_b [(1 - gamma) NLL_b + gamma/R sum_j (r_bj - r_b) NLL(y_bj)]."""
+    B = len(seqs_x)
+    if B < 1 or len(seqs_y) != B or len(baselines) != B:
+        raise ValueError('scst_batch: %d sources, %d references, %d baselines' % (B, len(seqs_y), len(baselines)))
+    if len(samples) % B or len(samples) < B or len(rewards) != len(samples):
+        raise ValueError('scst_batch: %d samples and %d rewards for %d sources' % (len(samples), len(rewards), B))
+    gamma = float(gamma)
+    if not 0. <= gamma <= 1.:
+        raise ValueError('gamma must be in [0, 1], got %r' % gamma)
+    R = len(samples) // B
+    xs, ys, w, cut = [], [], [], []
+    if gamma < 1.:
+        xs += list(seqs_x)
+        ys += list(seqs_y)
+        w += [1. - gamma] * B
+        cut += [False] * B
+    for q, s in enumerate(samples):
+        b = q // R
+        s = [int(t) for t in s]
+        ended = len(s) > 0 and s[-1] == 0
+        xs.append(seqs_x[b])
+        ys.append(s[:-1] if ended else s)
+        w.append(gamma * (float(rewards[q]) - float(baselines[b])) / R)
+        cut.append(not ended)
+    x, x_mask, y, y_mask = prepare_data(xs, ys)
+    for col, c in enumerate(cut):
+        if c:
+            y_mask[len(ys[col]), col] = 0.
+    return x, x_mask, y, y_mask, numpy.asarray(w, dtype='float32')
+
+
+def _check_scst(gamma, n_samples, maxlen, train_maxlen):
+    """the self-critical options of train(), checked before training starts (the sampling ones only when gamma > 0)"""
+    gamma = float(gamma)
+    if not 0. <= gamma <= 1.:
+        raise ValueError('rl_weight must be in [0, 1], got %r' % gamma)
+    if gamma == 0.:
+        return gamma, n_samples, maxlen
+    if int(n_samples) != n_samples or n_samples < 1:
+        raise ValueError('rl_samples must be an integer >= 1, got %r' % (n_samples,))
+    if int(maxlen) != maxlen or maxlen < 1 or maxlen > train_maxlen - 1:
+        raise ValueError('rl_maxlen must be an integer in [1, maxlen - 1 = %d] (prepare_data cuts longer targets), got %r'
+                         % (train_maxlen - 1, maxlen))
+    return gamma, int(n_samples), int(maxlen)
+
+
+def scst_step(tparams, f_init, f_next, options, f_grad_shared, seqs_x, seqs_y, gamma, n_samples, maxlen, seed, index_base,
+              global_batch=None):
+    """One self-critical gradient step (an addition beyond the reference; Rennie et al. 2017) on B sources seqs_x with
+    reference summaries seqs_y: R = n_samples unfiltered samples of each (sample_many, T = 1, UNK allowed), the greedy
+    summary as baseline (sample_many with top_k = 1), their ROUGE-L F against the references (ONE rouge_f call), then ONE
+    weighted f_grad_shared on scst_batch's columns with global_batch source pairs (default B).  Source b's rows are keyed by
+    index_base + b (sample_many).  -> (the weighted objective f_grad_shared returns, per-sample rewards [B*R], greedy
+    rewards [B]).  f_update is the caller's."""
+    B = len(seqs_x)
+    xs = [numpy.asarray(list(s) + [0], dtype='int64') for s in seqs_x]
+    R = n_samples
+    sam = sample_many(tparams, f_init, f_next, xs, options, n_samples=R, maxlen=maxlen, use_unk=True, seed=seed,
+                      index_base=index_base)
+    grd = sample_many(tparams, f_init, f_next, xs, options, n_samples=1, maxlen=maxlen, top_k=1, use_unk=True, seed=seed,
+                      index_base=index_base)
+    samples = [s for b in range(B) for s in sam[b][0]]
+    cands = [c for b in range(B) for c in sam[b][0] + grd[b][0]]       # per source: its R samples, then its greedy one
+    rl = rouge_f(cands, [list(s) for s in seqs_y], rows_per_ref=R + 1)[2].reshape(B, R + 1)
+    rewards, base = rl[:, :R].reshape(-1), rl[:, R]
+    x, x_mask, y, y_mask, w = scst_batch(seqs_x, seqs_y, samples, rewards, base, gamma)
+    cost = f_grad_shared(x, x_mask, y, y_mask, global_batch=B if global_batch is None else global_batch, weights=w)
+    return cost, rewards, base
+
+
 def gen_sample(tparams, f_init, f_next, x, options, trng=None, k=1, maxlen=30, stochastic=True, argmax=False,
                use_unk=False, kl_factor=0, ctx_factor=0, state_factor=0, no_repeat_ngram=0, min_len=0, _scorer_factory=None,
                _trace=None):
@@ -1859,18 +2017,27 @@ def train(dim_word=100, dim=1000, dim_att=100, encoder='gru', decoder='gru_cond'
           finish_after=10000000, dispFreq=100, decay_c=0., clip_c=-1., lrate=0.01, n_words=100000, maxlen=100,
           optimizer='adadelta', batch_size=16, valid_batch_size=16, saveto='model.npz', validFreq=1000,
           saveFreq=1000, sampleFreq=100, datasets=[], valid_datasets=[], dictionary='', use_dropout=False,
-          reload_=False, verbose=False, bucket_batches=0, save_optimizer_state=False, prefetch=2):
+          reload_=False, verbose=False, bucket_batches=0, save_optimizer_state=False, prefetch=2, rl_weight=0., rl_samples=4,
+          rl_maxlen=100, rl_seed=1234):
     """Same keyword surface, side effects (npz + options pickle, log lines) and return value as the reference's
     train() (nats.py:1230-1539).  Ours, all defaulting to the reference behaviour:
       bucket_batches        k > 0: the training iterator sorts k batches by source length before cutting them;
       save_optimizer_state  also write / reload `<saveto>.opt.npz` (the reference loses the accumulators, nats.py:1433);
-      prefetch              batches prepared ahead by a background thread (0 = inline as the reference).
+      prefetch              batches prepared ahead by a background thread (0 = inline as the reference);
+      rl_weight             gamma > 0: self-critical training (scst_step): every update mixes the maximum-likelihood
+                            cost, weighted 1 - gamma, with gamma x the policy gradient of the ROUGE-L of rl_samples
+                            samples per source (at most rl_maxlen words, <= maxlen - 1) against the greedy summary's,
+                            drawn with seed rl_seed.  Fine-tuning an ML model is reload_=True with rl_weight > 0.
     Under torchrun (one process per GPU, NCCL) every rank reads the same files; each global batch is sharded over the
     ranks, gradients are all-reduced once per update, rank 0 alone saves / samples / logs."""
     logging.basicConfig(level=logging.DEBUG, format="%(asctime)s: %(name)s: %(levelname)s: %(message)s")
     model_options = locals().copy()
-    for _k in ('save_optimizer_state', 'prefetch'):      # not part of the reference's option pickle
-        model_options.pop(_k)
+    for _k in ('save_optimizer_state', 'prefetch', 'rl_weight', 'rl_samples', 'rl_maxlen', 'rl_seed'):
+        model_options.pop(_k)                           # not part of the reference's option pickle
+    rl_weight, rl_samples, rl_maxlen = _check_scst(rl_weight, rl_samples, rl_maxlen, maxlen)
+    if int(rl_seed) != rl_seed or not 0 <= rl_seed < 2 ** 64:
+        raise ValueError('rl_seed must be an integer in [0, 2^64), got %r' % (rl_seed,))
+    scst = rl_weight > 0.
     rank, world = parallel.world()
     is_main = rank == 0
 
@@ -1922,7 +2089,8 @@ def train(dim_word=100, dim=1000, dim_att=100, encoder='gru', decoder='gru_cond'
         print('Reload optimizer state')
         load_optimizer_state(opt_path, f_grad_shared)
     # one workspace for the largest batch this run can produce: no regrowth (= no graph re-capture) later
-    grads.reserve(maxlen + 1, maxlen + 1, max(1, (batch_size + world - 1) // world))
+    per_rank = max(1, (batch_size + world - 1) // world)
+    grads.reserve(maxlen + 1, maxlen + 1, per_rank * (1 + rl_samples) if scst else per_rank)
     print('Optimization')
 
     history_errs = []
@@ -1946,16 +2114,19 @@ def train(dim_word=100, dim=1000, dim_att=100, encoder='gru', decoder='gru_cond'
             if world > 1:
                 bx, by, n_global = parallel.shard_batch(bx, by, rank, world)
             if len(bx) == 0:
-                yield None, None, None, None, n_global, 0
+                yield None, None, None, None, n_global, 0, None, None
                 continue
             x_, xm_, y_, ym_ = prepare_data(bx, by, maxlen=maxlen, n_words=n_words)
-            yield x_, xm_, y_, ym_, n_global, len(bx)
+            if scst:                                   # the pairs as prepare_data cut them
+                bx = [s[:maxlen - 1] if len(s) >= maxlen else s for s in bx]
+                by = [s[:maxlen - 1] if len(s) >= maxlen else s for s in by]
+            yield x_, xm_, y_, ym_, n_global, len(bx), bx, by
 
     uidx = 0
     estop = False
     for eidx in range(max_epochs):
         n_samples = 0
-        for x, x_mask, y, y_mask, n_global, n_local in _prefetched(_prepared(train_it), prefetch):
+        for x, x_mask, y, y_mask, n_global, n_local, bx, by in _prefetched(_prepared(train_it), prefetch):
             n_samples += n_global
             uidx += 1
             use_noise.set_value(1.)
@@ -1965,7 +2136,16 @@ def train(dim_word=100, dim=1000, dim_att=100, encoder='gru', decoder='gru_cond'
                 continue
 
             ud_start = time.time()
-            cost_v = f_grad_shared(x, x_mask, y, y_mask, global_batch=n_global)
+            if not scst or x is None:                  # (an empty shard only contributes zeros to the all-reduce)
+                cost_v = f_grad_shared(x, x_mask, y, y_mask, global_batch=n_global)
+                rl_s = rl_g = float('nan')
+            else:
+                # source b of this shard keys its draws by its place in the run: no (seed, step, row) repeats across
+                # updates or ranks (the shards are contiguous, parallel.shard)
+                base = (uidx - 1) * batch_size + rank * per_rank
+                cost_v, r_s, r_g = scst_step(tparams, f_init, f_next, model_options, f_grad_shared, bx, by, rl_weight,
+                                             rl_samples, rl_maxlen, rl_seed, base, global_batch=n_global)
+                rl_s, rl_g = float(r_s.mean()), float(r_g.mean())
             if verbose and clip_c > 0.:
                 norm_g = float(numpy.sqrt(grads.stats[0].item()))
             f_update(lrate)
@@ -1977,6 +2157,8 @@ def train(dim_word=100, dim=1000, dim_att=100, encoder='gru', decoder='gru_cond'
 
             if numpy.mod(uidx, dispFreq) == 0 and is_main:
                 logger.debug('Epoch {0} Update {1} Cost {2} UD {3}'.format(eidx, uidx, cost_v, ud))
+                if scst:
+                    logger.debug('ROUGE-L sample {0} greedy {1}'.format(rl_s, rl_g))
                 if verbose and clip_c > 0.:
                     logger.debug('Grad {0}'.format(norm_g))
 

@@ -3,6 +3,7 @@ hyper-parameter dictionary and the same fixed settings (maxlen=500, batch 20, fr
 location is an argument instead of a hard-coded /disk1/$USER path.
 
     python -m nats_b200.train_nats --data-dir DATA --model models/model.npz [--dim 600 ...]
+    python -m nats_b200.train_nats ... --reload --rl-weight 0.9      # self-critical fine-tuning of an ML model
     torchrun --nproc-per-node 8 -m nats_b200.train_nats ...      # data-parallel: each rank takes its shard of a batch
 """
 import argparse
@@ -37,6 +38,10 @@ def main(job_id, params):
                      saveFreq=10,
                      sampleFreq=10,
                      use_dropout=params['use-dropout'][0],
+                     rl_weight=params.get('rl-weight', [0.])[0],
+                     rl_samples=params.get('rl-samples', [4])[0],
+                     rl_maxlen=params.get('rl-maxlen', [100])[0],
+                     rl_seed=params.get('rl-seed', [1234])[0],
                      **({'finish_after': params['finish-after'][0]} if 'finish-after' in params else {}))
     return validerr
 
@@ -60,6 +65,11 @@ def _args():
     ap.add_argument('--batch-size', type=int, default=20)
     ap.add_argument('--finish-after', type=int, default=None)
     ap.add_argument('--reload', action='store_true')
+    ap.add_argument('--rl-weight', type=float, default=0.,
+                    help='gamma in [0, 1]: self-critical training on the ROUGE-L of sampled summaries (0 = off)')
+    ap.add_argument('--rl-samples', type=int, default=4, help='samples per source of a self-critical update')
+    ap.add_argument('--rl-maxlen', type=int, default=100, help='longest sampled summary (<= 499)')
+    ap.add_argument('--rl-seed', type=int, default=1234, help='seed of the self-critical samples')
     return ap.parse_args()
 
 
@@ -72,7 +82,8 @@ if __name__ == '__main__':
     p = {'data-dir': [a.data_dir], 'model': [a.model], 'train': a.train, 'valid': a.valid, 'dictionary': [a.dictionary],
          'dim_word': [a.dim_word], 'dim': [a.dim], 'dim_att': [a.dim_att], 'n-words': [a.n_words],
          'patience': [a.patience], 'optimizer': [a.optimizer], 'decay-c': [a.decay_c], 'clip-c': [a.clip_c],
-         'use-dropout': [False], 'learning-rate': [a.learning_rate], 'reload': [a.reload], 'batch-size': [a.batch_size]}
+         'use-dropout': [False], 'learning-rate': [a.learning_rate], 'reload': [a.reload], 'batch-size': [a.batch_size],
+         'rl-weight': [a.rl_weight], 'rl-samples': [a.rl_samples], 'rl-maxlen': [a.rl_maxlen], 'rl-seed': [a.rl_seed]}
     if a.finish_after is not None:
         p['finish-after'] = [a.finish_after]
     main(0, p)
